@@ -9,7 +9,7 @@ A "step" is one pass of the hot path (Filter::Evaluate -> one fused predicate + 
 compaction kernel) over one batch of `--rows` lineitem rows per GPU (default 1e9 = configs[1]
 of BASELINE.json; at N>1 each rank owns a contiguous row range: weak scaling, configs[4]
 shape; `--rows 1250000000` is configs[4]'s stated 10 B rows at N=8), inputs resident in HBM.
-Inputs (20 GB) are far larger than L2 (126 MB), so every step streams from HBM; no flush needed.
+Inputs (20 GB) are far larger than the H100's L2 (50 MB), so every step streams from HBM; no flush needed.
 
 `value`    = rows/s over all ranks, device-resident (CUDA events, max over ranks).
 `e2e`      = same metric through the C-ABI with HOST buffers (gdv_filter_evaluate(GDV_MEM_HOST)):
@@ -21,7 +21,7 @@ Inputs (20 GB) are far larger than L2 (126 MB), so every step streams from HBM; 
 `configs`  = (N=1 only) the other single-GPU workloads of BASELINE.json, each with rows/s, kernel
              ms, roofline fraction, a full-size check against an independent evaluation and the
              CPU arm's number:  q6_nulls (configs[1] with 1 % nulls per column), q1 (configs[2]:
-             eight-output projector, 2 % nulls, ~1e9 rows in chunks), str (configs[3]: string
+             eight-output projector, 2 % nulls, up to ~1e9 rows in chunks), str (configs[3]: string
              filter, 1e8 rows in 2 RecordBatches), ab_1m (configs[0]: a+b over a 1M-row batch).
 `cpu_baseline` = the CPU arm on this box's host cores.  Gandiva's LLVM JIT cannot be built in this
              image (no source under /root/reference, no LLVM), so the arm is
@@ -29,6 +29,8 @@ Inputs (20 GB) are far larger than L2 (126 MB), so every step streams from HBM; 
              g++ -O3 -march=native (AVX-512 where present), one pinned thread per hardware thread —
              plus `arrow_compute`: the same predicate through pyarrow.compute (not Gandiva either).
 `--impl reference` prints that CPU arm as its own line (same workload, same rows per step).
+`--dump-outputs DIR` writes the SelectionVector of the last timed step (what a caller of the timed path
+             receives) to DIR as float64 .npy files, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -49,12 +51,13 @@ IDX_BYTES = 4.0                # uint32 selection vector entries
 Q1_IN_BYTES = 8 + 3 * 16 + 3 * 8 + 4 + 8 / 8.0      # 8 columns + 8 validity bits
 Q1_OUT_BYTES = 2 * 16 + 6 * 8 + 8 / 8.0             # 8 outputs + 8 validity bits
 METRIC = "rows/sec (TPC-H Q6 filter over synthetic lineitem)"
+DUMP_MAX_ENTRIES = 2 << 20     # --dump-outputs: 16 MB of sampled indices + 16 MB of their positions
 
 
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps of the hot path (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--rows", type=int, default=int(os.environ.get("GDV_BENCH_ROWS", 0)),
@@ -84,14 +87,40 @@ def parse_args():
                     help="N>1, --gather push: filter each step's batch in this many row slices (wave-major global row "
                          "order) so that the NVLink push of slice j hides under the filter kernel of slice j+1 and only "
                          "the last slice's push is exposed.  Default 1 (one run per rank: the push of batch i hides under the filter of "
-                         "batch i+1, only the LAST batch's push is exposed).  Measured at N=2, 1.25e9 rows/GPU: 4 waves cost "
-                         "+0.23 ms per step (four kernel ramps instead of one) and take the last step from +0.28 ms to +0.09 ms "
-                         "— worth it for one isolated batch, not for a stream of batches (profiles/r02_multi_gpu.md)")
+                         "batch i+1, only the LAST batch's push is exposed).  More waves cost one kernel ramp each per step "
+                         "and shorten the exposed push of the last step: worth it for one isolated batch, not for a stream "
+                         "of batches")
     ap.add_argument("--push-ctas", type=int, default=8, help="--gather push: CTAs (256 threads) of the push kernel")
     ap.add_argument("--sm-reserve", type=int, default=-1,
                     help="SMs the filter leaves free for the push / NCCL kernels (default with N>1: 2, i.e. twelve "
                          "256-thread CTA slots for the eight push CTAs)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last step's SelectionVector (global row indices, on rank 0 "
+                         "at N>1) to DIR/selection_vector.npy as float64, with its length in DIR/selection_count.npy; "
+                         "vectors longer than %d entries are reduced to a fixed seeded sample whose positions go to "
+                         "DIR/selection_sample_positions.npy" % DUMP_MAX_ENTRIES)
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.gpus > 1 and (args.no_gather or args.gather != "push"):
+        ap.error("--dump-outputs with --gpus > 1 needs the SelectionVector on rank 0 (--gather push)")
+    return args
+
+
+def dump_selection(out_dir, idx):
+    """idx: the SelectionVector as int64 global row indices (a device tensor).  float64 holds every index below
+    2^53 exactly.  A longer vector is sampled at positions drawn with a fixed seed from its length, so that two
+    runs with the same arguments (the same inputs) sample the same positions."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = int(idx.numel())
+    np.save(os.path.join(out_dir, "selection_count.npy"), np.array([n], dtype=np.float64))
+    if n > DUMP_MAX_ENTRIES:
+        pos = np.sort(np.random.default_rng(20240601).choice(n, DUMP_MAX_ENTRIES, replace=False))
+        np.save(os.path.join(out_dir, "selection_sample_positions.npy"), pos.astype(np.float64))
+        idx = idx[torch.from_numpy(pos).to(idx.device)]
+    np.save(os.path.join(out_dir, "selection_vector.npy"), idx.cpu().numpy().astype(np.float64))
 
 
 def measured_peak_gbs():
@@ -99,7 +128,7 @@ def measured_peak_gbs():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not measured)"
 
 
 class ClockSampler:
@@ -336,7 +365,8 @@ def cfg_q6_nulls(ctx):
 
 
 def cfg_q1(ctx):
-    """configs[2]: eight-output Q1 projector, 2 % nulls per column, ~1e9 rows resident, evaluated in chunks."""
+    """configs[2]: eight-output Q1 projector, 2 % nulls per column, as many 64M-row chunks resident as HBM holds
+    (at most 15, ~1e9 rows; 12 on an 80 GB H100), evaluated chunk by chunk."""
     import pyarrow as pa
     torch, gandiva, cases = ctx["torch"], ctx["gandiva"], ctx["cases"]
     dev, stream, st = ctx["dev"], ctx["stream"], ctx["st"]
@@ -562,8 +592,8 @@ def cfg_ab_1m(ctx):
             "h2d_bytes_per_call": int(n * 8.25), "d2h_bytes_per_call": int(n * 4.125),
             "kernel_ms": ms, "device_resident_rows_per_s": n / ms * 1e3, "kernel": info["name"].rsplit("_", 1)[0],
             "regs": info["regs"], "algorithmic_bytes_per_row": 12.375,
-            "note": "1M rows = 12.4 MB: far below the ~100 MB a B200 needs in flight to reach its HBM roofline; the figure that "
-                    "matters here is the per-call latency next to the CPU arm's",
+            "note": "1M rows = 12.4 MB: a few microseconds of HBM traffic, less than the launch and copy overheads; the figure "
+                    "that matters here is the per-call latency next to the CPU arm's",
             "full_size_check": "ok: == oracle (python mirror and raw C-ABI host call)" if (ok and host_ok) else "FAILED",
             "_algo_bytes": algo}
 
@@ -647,7 +677,7 @@ def run_configs(ctx, only):
     for name in ("q6_nulls", "q1", "str", "ab_1m"):
         if name not in only:
             continue
-        if name == "q1":       # the Q1 inputs (84 GB) need the HBM the Q6 columns hold
+        if name == "q1":       # the Q1 inputs (85 B/row, up to 1e9 rows) need the HBM the Q6 columns hold
             for k in ("q6_cols", "out_idx"):
                 ctx[k] = None
             ctx["release"]()
@@ -709,8 +739,8 @@ def main():
     dev = torch.device("cuda", local_rank)
     torch.cuda.set_device(dev)
     # The process that feeds a GPU runs on the CPUs of the GPU's NUMA node (what a one-process-per-GPU launcher
-    # does with numactl / --cpunodebind): host batches are then allocated next to the link.  On the two-socket
-    # bench box the pageable e2e path varied 25-47 GB/s with the feeding thread left to float.  Undone before
+    # does with numactl / --cpunodebind): host batches are then allocated next to the link.  On a two-socket
+    # host the pageable e2e path varies widely with the feeding thread left to float.  Undone before
     # the CPU arms run, which use every core of the box.
     affinity0 = os.sched_getaffinity(0)
     numa_node, numa_cpus = gpu_numa_cpus(torch, dev)
@@ -733,6 +763,7 @@ def main():
     cfg = gandiva.Configuration(device=local_rank, rows_per_thread=args.rows_per_thread,
                                 block_threads=args.block_threads, sm_reserve=sm_reserve)
     filt, _ = q6_filter(gandiva, cases, cfg)
+    sm_count = torch.cuda.get_device_properties(dev).multi_processor_count
 
     # ---- inputs resident in HBM (generated on device; same stream as oracle/lineitem.h) -----
     cap_rows = n_nominal if world == 1 else (int(n_nominal * 1.05) // 64 + 1) * 64
@@ -751,8 +782,7 @@ def main():
     # ---- N>1 with the SelectionVector reassembled on rank 0: the root's shard is smaller ----------
     # Rank 0 does everything the other ranks do AND absorbs their runs: (N-1) x selectivity x 8 B per row
     # land in its HBM while its own filter streams 20 B per row, and an incoming write costs the memory
-    # system about twice what a streamed read does (measured: +0.39 ms per 1.27 GB at N=8, +0.16 ms per
-    # 0.54 GB at N=4, profiles/r02_multi_gpu.md).  With equal shards every step waits for rank 0; shards
+    # system about twice what a streamed read does (sharding.shard_rows_with_root's write_cost).  With equal shards every step waits for rank 0; shards
     # sized so that all ranks finish together keep the same total (N x rows) and the same global order.
     # The selectivity is measured by one calibration pass over the equal shards.
     shard_rows = [n_nominal] * world
@@ -849,7 +879,7 @@ def main():
                 ptr, cap, mode, cnt_ptr = ps.filter_target(g)
                 filt.evaluate_device(n, cols, ptr, cap, mode, st, cnt_ptr, sync=False, index_base=first_row)
                 # the last run of the job has no filter kernel to hide under: push it with the whole GPU
-                ps.after_filter(g, stream, ctas=(2 * 148 if i == k - 1 else 0))
+                ps.after_filter(g, stream, ctas=(2 * sm_count if i == k - 1 else 0))
             else:
                 at = 0
                 for j in range(waves):
@@ -859,7 +889,7 @@ def main():
                              (0, qty_full.data_ptr() + 8 * at, 0, 0)]
                     filt.evaluate_device(wave_rows[j], wcols, ptr, cap, mode, st, cnt_ptr, sync=False,
                                          index_base=wave_first[j])
-                    ps.after_filter(g, stream, ctas=(2 * 148 if (i == k - 1 and j == waves - 1) else 0), wave=j)
+                    ps.after_filter(g, stream, ctas=(2 * sm_count if (i == k - 1 and j == waves - 1) else 0), wave=j)
                     at += wave_rows[j]
             if events is not None and i + 1 < k:
                 events[i + 1].record(stream)
@@ -948,6 +978,10 @@ def main():
             del mask, idx
         except Exception as e:  # noqa: BLE001 - the bench line must still be printed
             full_check = "not run: %r" % (e,)
+        if args.dump_outputs:
+            idx = out_idx[:count].to(torch.int64)
+            dump_selection(args.dump_outputs, idx & 0xFFFFFFFF if idx_mode == "UINT32" else idx)
+            del idx
     if use_push:
         # outside the timed region: the last step's vector on rank 0 is complete and holds EXACTLY the
         # rows an independent torch evaluation of the predicate selects on every rank, in order:
@@ -972,6 +1006,8 @@ def main():
         if rank == 0:
             vec, total = ps.result(gstep["i"] - 1)
             ok = (total == total_selected) and not ps.overflowed()
+            if args.dump_outputs:
+                dump_selection(args.dump_outputs, vec[:total].to(torch.int64))
             pos = 0
             for j in range(waves):
                 for r in range(world):
@@ -1004,18 +1040,8 @@ def main():
     kernel_ms = kev[0].elapsed_time(kev[1]) / kreps
     achieved = algo_bytes / (kernel_ms * 1e-3) / 1e9
     info = filt.kernel_info
-    traffic = None
-    try:  # DRAM bytes per launch from the committed ncu --set full capture of this kernel/config
-        tj = json.load(open(os.path.join(ROOT, "profiles", "q6_filter_traffic.json")))
-        if int(tj["rows"]) == n and idx_mode == "UINT32":
-            traffic = float(tj["traffic_bytes_per_launch"])
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic,
-                "traffic_source": "profiles/q6_filter_traffic.json (ncu --set full capture of this kernel at this size, "
-                                  "committed; not re-measured in this run)" if traffic else None,
-                "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "kernel": info["name"].rsplit("_", 1)[0], "kernel_ms": kernel_ms,
                 "algorithmic_bytes_per_launch": algo_bytes, "regs": info["regs"],
                 "rows_per_thread": info["rows_per_thread"], "block_threads": info["block_threads"]}
@@ -1030,14 +1056,14 @@ def main():
     configs = None
     only = [x for x in (args.only.split(",") if args.only else ["q6_nulls", "q1", "str", "ab_1m"]) if x]
     if world == 1 and not args.no_configs:
-        holder = {"ship": ship, "disc": disc, "qty": qty}
+        holder = [ship_full, disc_full, qty_full]    # the Q6 columns (20 GB at 1e9 rows): Q1 needs that HBM
 
         def release():
             holder.clear()
         ctx = {"torch": torch, "gandiva": gandiva, "cases": cases, "dev": dev, "stream": stream, "st": st, "n": n,
                "local_rank": local_rank, "q6_cols": (ship, disc, qty), "out_idx": out_idx, "d_count": d_count,
                "release": release}
-        del ship, disc, qty, out_idx, bufs, cols
+        del ship, disc, qty, out_idx, bufs, cols, ship_full, disc_full, qty_full
         configs = run_configs(ctx, only)
 
     for tid in os.listdir("/proc/self/task"):      # threads created while bound inherited the mask

@@ -1,9 +1,9 @@
-// gdv_device_lib.cuh — device-side function library of the B200 expression engine.
+// gdv_device_lib.cuh — device-side function library of the H100 expression engine.
 //
 // Replaces the reference's precompiled-bitcode function library (BASELINE.json
 // north_star: "a device-side function library that replaces the precompiled-bitcode
 // function_registry").  This header is prepended to every kernel the fuser emits and
-// compiled by NVRTC for sm_100a at Projector/Filter::Make(); every function is
+// compiled by NVRTC for sm_90a at Projector/Filter::Make(); every function is
 // __forceinline__ so the per-row body becomes straight-line SASS.  It is also compiled
 // by nvcc in __graft_entry__.build() (static_kernels.cu includes it) as a syntax gate.
 //

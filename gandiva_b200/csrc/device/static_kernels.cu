@@ -1,6 +1,6 @@
 // static_kernels.cu — kernels that do not depend on the expression: the synthetic TPC-H
 // lineitem column generator used by bench.py / tests (SURVEY.md §8d concretisation) and an
-// L2 flush.  Compiled by nvcc to an sm_100a cubin at build time and embedded in
+// L2 flush.  Compiled by nvcc to an sm_90a cubin at build time and embedded in
 // libgandiva_b200.so; loaded through the driver API.  Including the device library here
 // also makes nvcc type-check every function in it (the build-time gate for code that
 // NVRTC otherwise only sees at Make()).
@@ -150,10 +150,9 @@ __device__ __forceinline__ void gdv_st_release_sys(u64* p, u64 v) {
 }
 #endif
 
-// Moves one index run into peer memory.  Measured on two B200s (profiles/r02_p2p_store_bench.txt): a
-// kernel's peer stores reach 579 GB/s with 16-byte stores (497 with 8-byte ones, copy engine 731), and
-// what limits a FEW CTAs is bytes in flight per thread: 8 CTAs x 256 threads move 320 GB/s with eight
-// 16-byte stores in flight per thread, 200 with four.  The CTAs are 256 threads wide because they must
+// Moves one index run into peer memory.  16-byte peer stores move more per instruction than 8-byte
+// ones, and what limits a FEW CTAs is bytes in flight per thread, so every thread keeps eight 16-byte
+// stores in flight (tools/p2p_store_bench.cu measures both on a pair of GPUs).  The CTAs are 256 threads wide because they must
 // fit the slots the persistent filter kernel (256-thread CTAs) leaves free (gdv_config_t.sm_reserve).
 template <typename T>
 __device__ __forceinline__ void gdv_copy_run_scalar(const T* __restrict__ src, T* dst, u64 n) {

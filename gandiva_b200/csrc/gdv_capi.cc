@@ -69,7 +69,7 @@ void gdv_config_default(gdv_config_t* cfg) {
   cfg->optimize = 1;
 }
 
-const char* gdv_version(void) { return "gandiva_b200 0.1 (sm_100a)"; }
+const char* gdv_version(void) { return "gandiva_b200 0.1 (sm_90a)"; }
 const char* gdv_last_error(void) { return tl_error.c_str(); }
 
 int32_t gdv_cuda_available(void) {

@@ -2158,8 +2158,8 @@ void MarkHoisted(const BodyGen& gen, const Node& cond, std::vector<ColumnSlot>* 
 }
 
 int PickRowsPerThread(int in_bytes, int out_bytes, KernelKind kind) {
-  // Measured on B200 (profiles/r01_sweeps.md): the map kernels want ~160-190 bytes of loads in
-  // flight per thread (add int32: R=16, Q6 predicate: R=8); the filter, whose tile is large
+  // The map kernels want ~160-190 bytes of loads in flight per thread to cover HBM latency
+  // (add int32: R=16, Q6 predicate: R=8); the filter, whose tile is large
   // and whose compaction tail needs registers, is best at R=2..4.
   (void)out_bytes;
   const int bytes = std::max(in_bytes, 1);
@@ -2193,8 +2193,8 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
     in_bytes += s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);
   }
   int R = spec.rows_per_thread > 0 ? std::min(spec.rows_per_thread, 8) : 2;
-  // String predicates are instruction-bound and stage bytes per warp in shared memory: 512 threads
-  // measured best on big batches (profiles/r01_string_filter.md); everything else runs 256.
+  // String predicates are instruction-bound and stage bytes per warp in shared memory: they run
+  // 512 threads on big batches; everything else runs 256.
   int BT = spec.block_threads > 0 ? spec.block_threads
                                   : (spec.kind == KernelKind::kFilter && n_varlen > 0 && spec.large_batch ? 512 : 256);
   if (BT % 32 != 0 || BT > 1024)
@@ -2507,7 +2507,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     KeyPlan plan;
     const int kBT = spec.block_threads > 0 ? spec.block_threads : 256;
     // chunks of 1024 rows per warp and tile: more rows per anchor drain and per tile-end barrier on
-    // big batches (Configuration.stages overrides), one on small ones (enough tiles for 148 SMs)
+    // big batches (Configuration.stages overrides), one on small ones (enough tiles for 132 SMs)
     const int kW = (spec.stages == 1 || spec.stages == 2 || spec.stages == 4) ? spec.stages : (spec.large_batch ? 2 : 1);
     if (kBT % 32 == 0 && kBT <= 1024 && kgen.PlanKey(*exprs[0]->root(), &plan)) {
       std::string kbody;
@@ -2576,9 +2576,8 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   for (const auto& e : exprs) out_bytes += std::max(e->result().type.width(), 1);
   if (spec.kind == KernelKind::kFilter) out_bytes = 0;
 
-  // The TMA loader is the default for wide-row projectors (measured on the Q1 projector, 166 B/row:
-  // 0.97 of the HBM copy peak at BT=256, R=2, 4 stages vs 0.73 for the best direct-load variant,
-  // profiles/r01_q1_tma_sweep.md).
+  // The TMA loader is the default for wide-row projectors (the Q1 projector, 166 B/row): bulk copies
+  // keep a whole tile per column in flight without spending registers on it.
   bool want_staged = spec.kind == KernelKind::kProject && spec.selection_mode == GDV_SEL_NONE &&
                      spec.loader != 1 && !slots.empty() && (spec.loader == 2 || in_bytes >= 48);
   for (const auto& sl : slots)
@@ -2592,8 +2591,8 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     while (p * 2 <= R) p *= 2;
     R = p;
   }
-  // String predicates are instruction-bound and stage bytes per warp in shared memory: 512 threads
-  // measured best on big batches (profiles/r01_string_filter.md); everything else runs 256.
+  // String predicates are instruction-bound and stage bytes per warp in shared memory: they run
+  // 512 threads on big batches; everything else runs 256.
   int BT = spec.block_threads > 0 ? spec.block_threads
                                   : (spec.kind == KernelKind::kFilter && n_varlen > 0 && spec.large_batch ? 512 : 256);
   if (BT % 32 != 0 || BT > 1024)
@@ -2633,7 +2632,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   // Each CTA tile (BT * R rows) of every input column is copied into a shared-memory stage by one
   // cp.async.bulk; S stages per CTA keep (S - 1) tiles in flight per CTA while one computes.
   // Picked by default for wide rows (>= 48 B of inputs), where the direct path runs out of
-  // registers before it has enough loads in flight (profiles/r01_configs_3_4.md).
+  // registers before it has enough loads in flight.
   bool staged = want_staged && (BT * R) % 128 == 0;
   std::vector<int> val_off(slots.size(), 0), vld_off(slots.size(), 0);
   int stage_total = 0, val_tx = 0, S = 0;
@@ -2863,7 +2862,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     // keep-mask is one ballot word, parked in lane k, so a chunk costs one register per thread
     // regardless of its size; loads are issued R steps at a time for memory-level parallelism.
     // Large tiles keep the number of look-back descriptors per launch small, which is what bounds
-    // ordered compaction at B200 bandwidth (DESIGN.md "Filter kernel").
+    // ordered compaction at HBM bandwidth (DESIGN.md "Filter kernel").
     const std::string IDX = SelCType(spec.selection_mode);
     const int NW = BT / 32;
     const int WT = NW * 1024 * W;
@@ -2887,8 +2886,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     if (n_varlen == 0) {
       // Fixed-width columns.  Every warp walks W consecutive 1024-row chunks per tile, so a
       // 32K-row tile needs 256 threads at W = 4 and eight small CTAs share an SM: while one sits in
-      // its tile-end barriers and look-back, seven keep streaming (measured on Q6, 1e9 rows:
-      // 256 threads x W=4 x R=4 2.95 ms against 3.25 ms for 1024 threads x W=1, profiles/r02_q6_sweeps.md).
+      // its tile-end barriers and look-back, seven keep streaming.
       src += "    #pragma unroll\n";
       src += "    for (int w = 0; w < " + sW + "; ++w) {\n";
       src += "      const i64 wbase = wbase0 + 1024 * w;\n";

@@ -81,11 +81,11 @@ const NvrtcApi& Nvrtc();
 // The device function library text (gdv_device_lib.cuh), embedded at build time.
 extern "C" const char gdv_device_lib_text[];
 extern "C" const unsigned long long gdv_device_lib_text_len;
-// Precompiled (nvcc, sm_100a) cubin of device/static_kernels.cu, embedded at build time.
+// Precompiled (nvcc, sm_90a) cubin of device/static_kernels.cu, embedded at build time.
 extern "C" const unsigned char gdv_static_kernels_cubin[];
 extern "C" const unsigned long long gdv_static_kernels_cubin_len;
 
-// Compile `source` (which #includes "gdv_device_lib.cuh") to an sm_100a cubin.
+// Compile `source` (which #includes "gdv_device_lib.cuh") to an sm_90a cubin.
 Status CompileToCubin(const std::string& source, const std::string& arch, bool optimize,
                       bool want_ptx, std::vector<char>* cubin, std::string* ptx,
                       std::string* log);

@@ -134,9 +134,9 @@ Status Device::MakeCurrent() const {
 }
 
 std::string Device::arch() const {
-  // This engine targets B200 only: sm_100a.  Other parts get their plain sm_XY so the
+  // This engine targets H100 only: sm_90a.  Other parts get their plain sm_XY so the
   // test-suite can still run on whatever GPU a developer has, without arch-specific code.
-  if (cc_major_ == 10 && cc_minor_ == 0) return "sm_100a";
+  if (cc_major_ == 9 && cc_minor_ == 0) return "sm_90a";
   return "sm_" + std::to_string(cc_major_) + std::to_string(cc_minor_);
 }
 
@@ -325,8 +325,8 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
   spec.name = placeholder;
   std::unique_ptr<CompiledKernel> k(new CompiledKernel());
   GDV_RETURN_NOT_OK(GenerateKernel(schema, exprs, spec, &k->gen));
-  // Compile for the device we will run on when one is visible, else for B200.
-  std::string arch = "sm_100a";
+  // Compile for the device we will run on when one is visible, else for H100.
+  std::string arch = "sm_90a";
   Device* dev = nullptr;
   if (Driver().loaded && Device::Get(cfg.device, &dev).ok()) arch = dev->arch();
   // name the kernel after its own text
@@ -1201,7 +1201,7 @@ Status Filter::KernelFor(int mode, bool nullable, bool large, CompiledKernel** o
     std::unique_ptr<CompiledKernel> k;
     std::vector<ExpressionPtr> exprs = {cond_};
     // Big batches want big tiles (few look-back descriptors), small ones enough tiles to occupy the
-    // 148 SMs: the fuser picks block size and chunks per warp from this flag (GenerateKernelImpl).
+    // 132 SMs: the fuser picks block size and chunks per warp from this flag (GenerateKernelImpl).
     Config cfg = cfg_;
     cfg.large_batch = large;
     GDV_RETURN_NOT_OK(BuildKernel(*schema_, exprs, KernelKind::kFilter, mode, nullable, cfg, &k));

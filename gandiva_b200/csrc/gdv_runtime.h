@@ -46,7 +46,7 @@ class Device {
   void SetPoolLimit(size_t bytes) { pool_limit_ = bytes; }
   size_t idle_bytes() const { return idle_bytes_; }
 
-  // Kernels of device/static_kernels.cu (embedded sm_100a cubin).
+  // Kernels of device/static_kernels.cu (embedded sm_90a cubin).
   Status StaticFunction(const char* name, CUfunction* out);
 
  private:

@@ -28,8 +28,8 @@ std::atomic<long long> g_staged_bytes{0};
 
 // ---- NUMA placement ---------------------------------------------------------------------------------------
 // The pinned ring and the copy threads belong on the NUMA node the GPU hangs off: a slot on the other socket
-// makes every DMA cross the socket interconnect, and copy threads floating over both sockets made the pageable
-// path vary between 25 and 47 GB/s from run to run on the two-socket bench box (profiles/r02_host_latency.md).
+// makes every DMA cross the socket interconnect, and copy threads floating over both sockets make the pageable
+// path's rate vary widely from run to run on a two-socket host.
 
 // CPUs of NUMA node `node` that this process may run on ("0-31,64-95" in sysfs); false if unreadable.
 bool NodeCpus(int node, cpu_set_t* out) {
@@ -122,9 +122,8 @@ class CopyPool {
   }
   // Copies in kChunk pieces that the calling thread and the workers CLAIM one at a time, so the call
   // never waits for a worker to wake up: a worker that is asleep (or descheduled) simply claims nothing
-  // and the caller copies those pieces itself.  (The first version gave every thread a fixed slice and
-  // waited for all of them; waking seven sleeping workers cost ~1 ms on the bench box — the D2H half of a
-  // 1M-row a+b call took 1.1 ms against 0.11 ms for the H2D half, profiles/r02_host_latency.md.)
+  // and the caller copies those pieces itself: waiting for seven sleeping workers to wake can cost more
+  // than the copy of a 1M-row column.
   void Copy(void* dst, const void* src, size_t bytes) {
     if (bytes < 2 * kChunk || workers_ == 0) {
       std::memcpy(dst, src, bytes);
@@ -133,8 +132,7 @@ class CopyPool {
     std::lock_guard<std::mutex> one_caller(caller_mu_);
     const unsigned long long e = (ticket_.load(std::memory_order_relaxed) >> 32) + 1;
     // Full ring slots (the pieces of a bulk transfer) go in 1 MB pieces: memcpy then takes its streaming
-    // (non-temporal store) path and the 8 threads each get one piece — 46.9 GB/s pageable->device on the
-    // bench box against 37.7 GB/s in 256 KB pieces (profiles/r02_host_latency.md).  Smaller copies (one
+    // (non-temporal store) path and the 8 threads each get one piece.  Smaller copies (one
     // column of a 1M-row batch) go in 256 KB pieces so that every thread has something to claim.
     const size_t chunk = chunk_override_ != 0 ? chunk_override_ : (bytes >= kSlotBytes ? 4 * kChunk : kChunk);
     const unsigned nchunks = static_cast<unsigned>((bytes + chunk - 1) / chunk);

@@ -27,7 +27,7 @@ def shard_rows_with_root(total_rows: int, world: int, selectivity: float, bytes_
     """Row counts per rank (contiguous ranges, in rank order, summing to total_rows) for a Filter whose
     SelectionVector is reassembled on rank 0.  The root streams its own rows AND absorbs the other ranks'
     runs — (world-1) x selectivity x index_bytes per row of a shard, each incoming byte costing the memory
-    system about `write_cost` streamed bytes (measured 2.0 on B200, DESIGN.md §4) — so with equal ranges every
+    system about `write_cost` streamed bytes (2.0 by default, DESIGN.md §4) — so with equal ranges every
     step waits for it.  The root's range is shortened until all ranks finish together.  Every range but the
     last is a multiple of `align` rows (no two shards share a validity-bitmap word)."""
     if world <= 1:

@@ -1,5 +1,5 @@
 /*
- * gandiva_b200.h — C-ABI of the B200-native expression engine.
+ * gandiva_b200.h — C-ABI of the H100-native expression engine.
  *
  * This is the drop-in boundary for the Gandiva hot path (Projector / Filter
  * Make + Evaluate over Arrow buffers).  Everything here is `extern "C"`, plain

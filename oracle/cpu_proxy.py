@@ -14,6 +14,7 @@ import ctypes as C
 import hashlib
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -36,9 +37,21 @@ def _cpu_key() -> str:
 
 
 def build() -> str:
-    path = os.path.join(_DIR, "libgdv_cpu_proxy_%s.so" % _cpu_key())
+    """Path of the library for this CPU, compiled first if missing.  A tree that is read-only (an installed
+    or shared checkout) gets its library in a per-user temporary directory instead of oracle/_proxy/."""
+    name = "libgdv_cpu_proxy_%s.so" % _cpu_key()
+    path = os.path.join(_DIR, name)
     if not os.path.exists(path):
-        os.makedirs(_DIR, exist_ok=True)
+        try:
+            os.makedirs(_DIR, exist_ok=True)
+            writable = os.access(_DIR, os.W_OK)
+        except OSError:
+            writable = False
+        if not writable:
+            tmp_dir = os.path.join(tempfile.gettempdir(), "gdv_cpu_proxy_%d" % os.getuid())
+            os.makedirs(tmp_dir, exist_ok=True)
+            path = os.path.join(tmp_dir, name)
+    if not os.path.exists(path):
         tmp = path + ".tmp%d" % os.getpid()
         subprocess.check_call(["g++"] + CXXFLAGS + [os.path.join(_HERE, "cpu_proxy.cc"), "-o", tmp])
         os.replace(tmp, path)

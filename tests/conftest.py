@@ -25,7 +25,7 @@ if os.path.isdir(_CUBIN_CACHE) and os.environ.get("GDV_EMU") != "1":
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # build the native libraries once per session if they are missing (in-tree .so files
     # normally travel with the snapshot)
     import importlib.util

@@ -263,7 +263,7 @@ CUresult cuDeviceGet(CUdevice* d, int ordinal) {
 CUresult cuDeviceGetAttribute(int* v, CUdevice_attribute a, CUdevice) {
   switch (a) {
     case CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT: *v = g_sm_count; break;
-    case CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MAJOR: *v = 10; break;
+    case CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MAJOR: *v = 9; break;
     case CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MINOR: *v = 0; break;
     case CU_DEVICE_ATTRIBUTE_MAX_SHARED_MEMORY_PER_BLOCK_OPTIN: *v = 227 * 1024; break;
     case CU_DEVICE_ATTRIBUTE_WARP_SIZE: *v = 32; break;

@@ -25,7 +25,7 @@ def test_header_symbols_exported():
 
 def test_library_loads_without_gpu(gandiva):
     assert gandiva.lib.gdv_version().startswith(b"gandiva_b200")
-    # never raises; 0 on this CPU-only container, 1 on the B200 box
+    # never raises; 0 on this CPU-only container, 1 on a GPU machine
     assert gandiva.lib.gdv_cuda_available() in (0, 1)
 
 

@@ -6,7 +6,7 @@ stand-in libcuda.so.1 / libnvrtc.so.12 in front of the real ones; the generated 
 compiled for the host against tests/emu/gdv_emu.h and every CUDA thread is a fiber.  The simulator
 is test infrastructure only: it checks kernel *logic* (tails, validity windows, ballots, scans,
 look-back, staging protocols, function semantics) against the oracle without a GPU; the `-m gpu`
-run of the very same test functions on the B200 box stays the parity gate.
+run of the very same test functions on the H100 stays the parity gate.
 
 Every `gpu`-marked test runs (about a minute on 8 cores, compiled kernels are cached under
 /tmp/gdv_emu_cache_<uid>, outside the tree); GDV_EMU_SELECT=<pytest -k expression> narrows it while developing."""

@@ -2,7 +2,7 @@
 grown at random over the registered function signatures, if/else, Kleene and/or, IN and literals,
 lowered by the fuser to one kernel per Projector / Filter, and compared with the scalar oracle on
 random batches with nulls — bit-exact, validity included.  Seeds are fixed: a failure names the
-seed that reproduces it.  Runs on the B200 (`-m gpu`) and, through tests/test_emu.py, under the
+seed that reproduces it.  Runs on the H100 (`-m gpu`) and, through tests/test_emu.py, under the
 functional simulator on a CPU-only box."""
 import numpy as np
 import pyarrow as pa
@@ -26,7 +26,7 @@ TYPES = [I32, I64, F32, F64, B, S, BIN, D64, TS, T32, D32]
 SKIP = {"divide", "div", "like", "ilike", "regexp_matches", "regexp_like", "concat", "concatOperator", "sqrt", "castDECIMAL", "split_part",
         "repeat", "space", "reverse", "lpad", "rpad", "replace",
         "power", "pow", "cot", "sinh", "cosh",   # same as exp below: inf arrives quickly
-        "exp",   # overflows to inf on the random doubles; inf - inf then makes a hardware NaN whose sign differs between x86 and sm_100a
+        "exp",   # overflows to inf on the random doubles; inf - inf then makes a hardware NaN whose sign differs between x86 and sm_90a
         "timestampaddMonth", "timestampaddQuarter", "timestampaddYear", "mod", "modulo",
         "factorial",   # raises outside 0..20 (dedicated tests)
         "initcap",   # a lazy case map that may not be narrowed from the left afterwards (dedicated test)

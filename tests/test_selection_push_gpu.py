@@ -139,8 +139,8 @@ import os  # noqa: E402
 
 # Several virtual ranks on ONE device wait for each other inside kernels: that needs the kernels of several
 # streams to be resident at the same time, which CUDA does not promise (and the CPU simulator runs one kernel
-# at a time).  It works on B200 (tools/r02_call6.sh runs it under a timeout) but a test that could hang a
-# box is opt-in; the real multi-GPU path is tests/peer_push_worker.py.
+# at a time).  A test that could hang a GPU is therefore opt-in; the real multi-GPU path is
+# tests/peer_push_worker.py.
 needs_concurrency = pytest.mark.skipif(devmem.EMU or os.environ.get("GDV_TEST_VIRTUAL_RANKS") != "1",
                                        reason="opt-in: GDV_TEST_VIRTUAL_RANKS=1 (ranks wait for each other on one device)")
 

@@ -1,8 +1,8 @@
-// p2p_store_bench.cu — how fast can ONE B200 store an index run into a peer GPU's HBM over NVLink,
+// p2p_store_bench.cu — how fast can ONE H100 store an index run into a peer GPU's HBM over NVLink,
 // as a function of store width, CTAs and bytes in flight?  Decides the shape of gdv_sel_push
 // (csrc/device/static_kernels.cu).  Single process, two devices, peer access enabled.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a tools/p2p_store_bench.cu -o tools/_bin/p2p_store_bench
-//   gpurun --gpus 2 -- ./tools/_bin/p2p_store_bench
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a tools/p2p_store_bench.cu -o tools/_bin/p2p_store_bench
+//   ./tools/_bin/p2p_store_bench          (on a machine with two GPUs)
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -64,7 +64,7 @@ int main() {
     CK(cudaEventElapsedTime(&ms, e0, e1));
     printf("%-44s peer   %7.3f ms  %7.1f GB/s\n", "cudaMemcpyPeerAsync (copy engine)", ms / 5, bytes / (ms / 5) / 1e6);
   }
-  const int ctas_list[] = {4, 8, 16, 32, 148, 296};
+  const int ctas_list[] = {4, 8, 16, 32, 132, 264};
   for (int ctas : ctas_list) {
     for (int bt : {256, 1024}) {
       snprintf(name, sizeof(name), "u64 x8 strided, %3d CTAs x %4d", ctas, bt);

@@ -1,4 +1,4 @@
-"""Fill gandiva_b200/_cubin_cache with sm_100a cubins of kernels the `-m gpu` suite makes, on a box
+"""Fill gandiva_b200/_cubin_cache with sm_90a cubins of kernels the `-m gpu` suite makes, on a box
 WITHOUT a GPU.  NVRTC needs no device: the suite is simply run here with GDV_CUBIN_CACHE_DIR set and
 GDV_EAGER_NONULL=1 (the no-null variants are built at Make() too); every Make() compiles with the
 real NVRTC and lands in the cache, every test then fails at its first Evaluate (no driver), which is

@@ -1,7 +1,7 @@
 """gdv_sel_push on ONE GPU: a single rank in wave mode copies its own run into the vector (HBM -> HBM), which is the
-kernel's copy loop without the link.  Timed with CUDA events for 8 and 296 CTAs; run under
-`ncu -k gdv_sel_push --set full` for the instruction / memory profile of that loop (profiles/r02_sel_push_local.*).
-The NVLink side of the same loop is tools/p2p_store_bench.cu (profiles/r02_p2p_store_bench.txt)."""
+kernel's copy loop without the link.  Timed with CUDA events for 8 and 264 CTAs (two per H100 SM); run under
+`ncu -k gdv_sel_push --set full` for the instruction / memory profile of that loop.
+The NVLink side of the same loop is tools/p2p_store_bench.cu."""
 import os
 import sys
 
@@ -22,7 +22,7 @@ base = torch.zeros(1, dtype=torch.int64, device=dev)
 total = torch.zeros(1, dtype=torch.int64, device=dev)
 stream = torch.cuda.current_stream().cuda_stream
 issued, seq = 0, 0
-for ctas in (8, 8, 296, 296):
+for ctas in (8, 8, 264, 264):
     issued += ctas
     seq += 1
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -1,7 +1,7 @@
 """Static SASS facts of the kernels the bench configs use (no GPU needed: NVRTC + cuobjdump):
 registers, stack, SASS instruction count and the mnemonics that show how data moves (UBLKCP = TMA
 bulk copy, SYNCS = mbarrier, LDGSTS = cp.async, LDG.E.128 / .64, VOTE / SHFL / BAR).
-  python tools/sass_stats.py > profiles/<name>.md"""
+  python tools/sass_stats.py > sass_stats.md"""
 import collections
 import os
 import re
