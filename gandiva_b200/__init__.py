@@ -74,6 +74,13 @@ class gdv_column_t(C.Structure):
                 ("offset", C.c_int64), ("var_data_size", C.c_int64)]
 
 
+class gdv_dictionary_t(C.Structure):
+    """The dictionary of a dictionary-encoded column (include/gandiva_b200.h): the column's
+    gdv_column_t holds validity + indices, and its var_data points at one of these."""
+    _fields_ = [("validity", C.c_void_p), ("offsets", C.c_void_p), ("data", C.c_void_p),
+                ("offset", C.c_int64), ("length", C.c_int64), ("data_size", C.c_int64)]
+
+
 class gdv_batch_t(C.Structure):
     _fields_ = [("num_rows", C.c_int64), ("num_columns", C.c_int32), ("mem_space", C.c_int32),
                 ("columns", C.POINTER(gdv_column_t))]
@@ -209,7 +216,14 @@ def launch_count() -> int:
 _UNIT = {"s": 0, "ms": 1, "us": 2, "ns": 3}
 
 
+GDV_TYPE_DICTIONARY = 29
+GDV_DICT_ORDERED = 0x100
+
+
 def _to_c_type(t: pa.DataType) -> gdv_type_t:
+    if pa.types.is_dictionary(t):
+        return gdv_type_t(GDV_TYPE_DICTIONARY, int(t.index_type.id) | (GDV_DICT_ORDERED if t.ordered else 0),
+                          int(t.value_type.id))
     if pa.types.is_decimal128(t):
         return gdv_type_t(int(t.id), t.precision, t.scale)
     if pa.types.is_timestamp(t) or pa.types.is_time32(t) or pa.types.is_time64(t):
@@ -225,6 +239,8 @@ def _from_c_type(t: gdv_type_t) -> pa.DataType:
               17: pa.date64()}
     if tid in simple:
         return simple[tid]
+    if tid == GDV_TYPE_DICTIONARY:
+        return pa.dictionary(simple[t.precision & 0xff], simple[t.scale], bool(t.precision & GDV_DICT_ORDERED))
     unit = {0: "s", 1: "ms", 2: "us", 3: "ns"}.get(t.precision, "ms")
     if tid == 18:
         return pa.timestamp(unit)
@@ -546,6 +562,24 @@ class SelectionVector:
 
 
 # ---- batch marshalling -------------------------------------------------------------------
+def _dictionary_to_c(d: pa.Array) -> gdv_dictionary_t:
+    """A utf8 / binary dictionary -> gdv_dictionary_t over its own buffers (no copies).  The
+    struct keeps the arrays it points into alive."""
+    bufs = d.buffers()
+    if len(bufs) != 3:
+        raise pa.ArrowNotImplementedError("dictionary of type %s: only utf8 and binary dictionaries are supported"
+                                          % d.type)
+    c = gdv_dictionary_t()
+    c.validity = bufs[0].address if bufs[0] is not None and d.null_count > 0 else None
+    c.offsets = bufs[1].address if bufs[1] is not None else None
+    c.data = bufs[2].address if bufs[2] is not None else None
+    c.offset = d.offset
+    c.length = len(d)
+    c.data_size = bufs[2].size if bufs[2] is not None else 0
+    c._keep = (d, bufs)
+    return c
+
+
 def _batch_to_c(batch: pa.RecordBatch):
     """RecordBatch -> gdv_batch_t over the batch's own buffers (no copies)."""
     cols = (gdv_column_t * max(batch.num_columns, 1))()
@@ -558,7 +592,13 @@ def _batch_to_c(batch: pa.RecordBatch):
         # a bitmap without any cleared bit is passed as "no validity" (selects the no-null kernel)
         c.validity = bufs[0].address if bufs[0] is not None and arr.null_count > 0 else None
         t = arr.type
-        if pa.types.is_string(t) or pa.types.is_binary(t):
+        if pa.types.is_dictionary(t):
+            # indices like a fixed-width column; var_data -> the dictionary (zero copy)
+            c.values = bufs[1].address if bufs[1] is not None else None
+            d = _dictionary_to_c(arr.dictionary)
+            keep.append(d)
+            c.var_data = C.addressof(d)
+        elif pa.types.is_string(t) or pa.types.is_binary(t):
             c.values = bufs[1].address if bufs[1] is not None else None
             c.var_data = bufs[2].address if len(bufs) > 2 and bufs[2] is not None else None
             c.var_data_size = bufs[2].size if len(bufs) > 2 and bufs[2] is not None else 0
@@ -567,6 +607,14 @@ def _batch_to_c(batch: pa.RecordBatch):
         c.offset = arr.offset
     b = gdv_batch_t(batch.num_rows, batch.num_columns, GDV_MEM_HOST, cols)
     return b, (cols, keep)
+
+
+def _var_ptr(var):
+    """var_data of a device column: the bytes of a utf8 / binary column, or a gdv_dictionary_t (with
+    device pointers) for a dictionary-encoded one."""
+    if isinstance(var, gdv_dictionary_t):
+        return C.addressof(var)
+    return var or None
 
 
 class _SchemaHandle:
@@ -601,6 +649,8 @@ def _kernel_info(fn, handle, attr_fn=None) -> dict:
             "rows_per_thread": rpt.value, "block_threads": bt.value}
     if attr_fn is not None:
         keys = ["staged", "stages", "dynamic_smem", "cta_tile_rows", "tile_rows", "nullable"]
+        if attr_fn is lib.gdv_filter_kernel_attr:
+            keys.append("dictionary_first")
         if regs.value >= 0:
             keys.append("blocks_per_sm")
         for key in keys:
@@ -681,14 +731,15 @@ class Projector:
     # -- device-resident path (bench / multi-GPU): raw pointers in HBM, caller-owned stream ----
     def evaluate_device(self, num_rows: int, columns: Sequence[tuple], outputs: Sequence[tuple],
                         stream: int = 0, selection: tuple | None = None, sync: bool = False) -> None:
-        """columns: per schema field (validity_ptr|0, values_ptr, var_data_ptr|0, offset);
+        """columns: per schema field (validity_ptr|0, values_ptr, var_data_ptr|0, offset), where a
+        dictionary-encoded column passes its indices as values and a gdv_dictionary_t as var_data;
         outputs: per expression (validity_ptr|0, values_ptr); selection: (ptr, num_slots) or
         (ptr, max_slots, d_count_ptr): the slot count is read from device memory (the d_count a
         Filter.evaluate_device(..., sync=False) wrote on the same stream), no host round trip."""
         cols = (gdv_column_t * max(len(columns), 1))()
         for i, (vld, val, var, off) in enumerate(columns):
             cols[i].validity, cols[i].values, cols[i].var_data, cols[i].offset = \
-                (vld or None), (val or None), (var or None), off
+                (vld or None), (val or None), _var_ptr(var), off
         cb = gdv_batch_t(num_rows, len(columns), GDV_MEM_DEVICE, cols)
         outs = (gdv_out_column_t * max(len(outputs), 1))()
         for i, (vld, val) in enumerate(outputs):
@@ -757,7 +808,7 @@ class Filter:
         cols = (gdv_column_t * max(len(columns), 1))()
         for i, (vld, val, var, off) in enumerate(columns):
             cols[i].validity, cols[i].values, cols[i].var_data, cols[i].offset = \
-                (vld or None), (val or None), (var or None), off
+                (vld or None), (val or None), _var_ptr(var), off
         cb = gdv_batch_t(num_rows, len(columns), GDV_MEM_DEVICE, cols)
         sel = gdv_selection_t(out_indices, max_slots, 0, _ensure_selection_mode(mode), GDV_MEM_DEVICE,
                               index_base)

@@ -208,6 +208,24 @@ GDV_DEV bool gdv_ldbit(const u8* p, u32 sh, i64 i) {
   const i64 b = i + (i64)sh;
   return ((p[b >> 3] >> (u32)(b & 7)) & 1u) != 0u;
 }
+// Row of a dictionary-encoded column: the view of entry `ix` of a utf8 / binary dictionary
+// (offsets from the dictionary's own offset on, its bytes, validity words + bit shift, length).
+// *ok = the entry is valid.  An index outside [0, dlen) is invalid Arrow input: the row reads as
+// null and nothing of the dictionary is loaded.  The dictionary is small and shared by many rows:
+// its loads go through the read-only cache.
+GDV_DEV gdv_str gdv_dict_view(const i32* dof, const u8* dat, const u32* dvl, u32 dvs, i64 dlen, i64 ix,
+                              bool* ok) {
+  const bool in = (u64)ix < (u64)dlen;
+  i32 a = 0, b = 0;
+  bool v = false;
+  if (in) {
+    a = __ldg(dof + ix);
+    b = __ldg(dof + ix + 1);
+    v = dvl == nullptr || ((__ldg(dvl + ((ix + (i64)dvs) >> 5)) >> (u32)((ix + (i64)dvs) & 31)) & 1u) != 0u;
+  }
+  *ok = v;
+  return gdv_make_str(dat + a, b - a);
+}
 // The 32 bitmap bits of rows [rb, rb + 32), rb % 32 == 0, of a bitmap whose row 0 is bit `sh` of the
 // 4-byte aligned word *p; rows >= n read as 0 and no byte past the one that holds row n - 1 is touched.
 // (Filter epilogue: one word per lane and 1024-row chunk, ColumnSlot::hoist.)

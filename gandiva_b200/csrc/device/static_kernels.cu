@@ -126,6 +126,185 @@ gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit) {
   }
 }
 
+// ---- dictionary-first Filter (DESIGN.md §3.6) -----------------------------------------------------
+// A Filter whose condition reads one dictionary-encoded column only, and is never true when that
+// column is null, has been evaluated once per dictionary ENTRY (bit e of `bits` = the condition holds
+// for entry e).  This kernel streams the indices and their validity and keeps row r iff its index is
+// valid, lies in [0, dlen) and its entry's bit is set -- the ordered compaction is the fused filter
+// kernel's (gdv_filter_expr_*, §3.3): persistent 256-thread CTAs take W-chunk tiles from a ticket,
+// step k's keep-mask is one ballot parked in lane k, warp and CTA scans, decoupled look-back.
+// The entry bitmap is copied into shared memory when `smem_words` != 0 (dictionaries of up to
+// GDV_DICT_SMEM_ENTRIES entries), else it is read through L1 / L2.
+#define GDV_DICT_SMEM_ENTRIES 65536
+template <typename IT, int W>
+__device__ __forceinline__ void gdv_dict_filter_body(const IT* idx, const u32* vld, u32 vsh, const u32* bits,
+                                                     i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx,
+                                                     int out_width, u64* out_count, u64* tile_state, u64* ticket,
+                                                     i64 out_cap, u32* s_bits, u32* s_wcount, i64& s_tile, u64& s_excl) {
+  constexpr int NW = 8;  // warps per CTA (256 threads)
+  constexpr int R = 8;   // 32-row steps whose index loads are in flight together
+  constexpr i64 WT = (i64)NW * 1024 * W;
+  const u32 lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+  for (int i = (int)threadIdx.x; i < smem_words; i += (int)blockDim.x) s_bits[i] = __ldg(bits + i);
+  __syncthreads();
+  const u32* eb = smem_words != 0 ? s_bits : bits;
+  const i64 n_tiles = (n + WT - 1) / WT;
+  const u32 lt = gdv_lanemask_lt();
+  while (true) {
+    if (threadIdx.x == 0) s_tile = (i64)atomicAdd(ticket, 1ull);
+    __syncthreads();
+    const i64 tile = s_tile;
+    if (tile >= n_tiles) break;
+    const i64 wbase0 = tile * WT + (i64)wid * (1024 * W);
+    u32 mymask[W];
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      const i64 wbase = wbase0 + 1024 * w;
+      u32 cur = 0u;
+#pragma unroll 1
+      for (int g = 0; g < 32; g += R) {
+        const i64 base = wbase + 32 * g;
+        if (base >= n) break;
+        i64 x[R];
+        if (base + 32 * R <= n) {
+#pragma unroll
+          for (int k = 0; k < R; ++k) x[k] = (i64)gdv_ldp(idx + base + 32 * k + lane);
+        } else {
+#pragma unroll
+          for (int k = 0; k < R; ++k) {
+            const i64 s = base + 32 * k + (i64)lane;
+            x[k] = s < n ? (i64)gdv_ldp(idx + s) : -1ll;
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < R; ++k) {
+          // an index outside [0, dlen) is invalid Arrow input: the row reads as null, never kept
+          const bool keep = (u64)x[k] < (u64)dlen && ((eb[x[k] >> 5] >> (u32)(x[k] & 31)) & 1u) != 0u;
+          const u32 m = __ballot_sync(GDV_FULL, keep);
+          if (lane == (u32)(g + k)) cur = m;
+        }
+      }
+      mymask[w] = cur;
+    }
+    if (vld != nullptr) {  // null indices: one validity word per lane and chunk
+#pragma unroll
+      for (int w = 0; w < W; ++w) {
+        const i64 rb = wbase0 + 1024 * w + 32 * (i64)lane;
+        if (rb < n) mymask[w] &= gdv_ldwin_rows(vld, vsh, rb, n);
+      }
+    }
+    u32 step_excl[W];
+    u32 run = 0u;
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      const u32 c = (u32)__popc(mymask[w]);
+      u32 incl = c;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const u32 t = __shfl_up_sync(GDV_FULL, incl, o);
+        if (lane >= (u32)o) incl += t;
+      }
+      step_excl[w] = run + incl - c;
+      run += __shfl_sync(GDV_FULL, incl, 31);
+    }
+    if (lane == 0u) s_wcount[wid] = run;
+    __syncthreads();
+    if (wid == 0u) {
+      const u32 wc = lane < (u32)NW ? s_wcount[lane] : 0u;
+      u32 winc = wc;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const u32 t = __shfl_up_sync(GDV_FULL, winc, o);
+        if (lane >= (u32)o) winc += t;
+      }
+      const u32 total = __shfl_sync(GDV_FULL, winc, 31);
+      if (lane < (u32)NW) s_wcount[lane] = winc - wc;
+      const u64 excl = gdv_tile_exclusive_prefix(tile_state, tile, (u64)total, lane);
+      if (lane == 0u) {
+        s_excl = excl;
+        if (tile == n_tiles - 1) *out_count = excl + (u64)total;
+      }
+    }
+    __syncthreads();
+    const u64 wpos = s_excl + (u64)s_wcount[wid];
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      if (__ballot_sync(GDV_FULL, mymask[w] != 0u) == 0u) continue;
+#pragma unroll 1
+      for (int k = 0; k < 32; ++k) {
+        const u32 m = __shfl_sync(GDV_FULL, mymask[w], k);
+        if (m == 0u) continue;  // warp-uniform
+        const u64 pos = wpos + (u64)__shfl_sync(GDV_FULL, step_excl[w], k) + (u64)__popc(m & lt);
+        if (((m >> lane) & 1u) && pos < (u64)out_cap) {
+          const i64 row = row_base + wbase0 + 1024 * w + 32 * k + (i64)lane;
+          if (out_width == 2) static_cast<u16*>(out_idx)[pos] = (u16)row;
+          else if (out_width == 4) static_cast<u32*>(out_idx)[pos] = (u32)row;
+          else static_cast<u64*>(out_idx)[pos] = (u64)row;
+        }
+      }
+    }
+  }
+}
+
+// One kernel per index type and chunks per warp (W = 4 on batches of >= 32 M rows, as the fused filter).
+// The shared variables live in the kernels, not in the template: one copy per kernel.
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i8_w1(const i8* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i8, 1>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i8_w4(const i8* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i8, 4>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i16_w1(const i16* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i16, 1>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i16_w4(const i16* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i16, 4>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i32_w1(const i32* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i32, 1>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i32_w4(const i32* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i32, 4>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i64_w1(const i64* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i64, 1>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+extern "C" __global__ void __launch_bounds__(256) gdv_dict_filter_i64_w4(const i64* idx, const u32* vld, u32 vsh, const u32* bits, i64 dlen, int smem_words, i64 n, i64 row_base, void* out_idx, int out_width, u64* out_count, u64* tile_state, u64* ticket, i64 out_cap) {
+  extern __shared__ uint4 gdv_smem[];
+  __shared__ u32 s_wcount[8];
+  __shared__ i64 s_tile;
+  __shared__ u64 s_excl;
+  gdv_dict_filter_body<i64, 4>(idx, vld, vsh, bits, dlen, smem_words, n, row_base, out_idx, out_width, out_count, tile_state, ticket, out_cap, reinterpret_cast<u32*>(gdv_smem), s_wcount, s_tile, s_excl);
+}
+
 // ---- SelectionVector reassembly across row-range shards (DESIGN.md "Multi-GPU") ------------
 // One process per GPU filters its row range into a LOCAL index run (global row numbers).  This
 // kernel, launched on a side stream next to the following batch's filter kernel, moves the run

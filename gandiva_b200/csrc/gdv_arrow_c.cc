@@ -116,6 +116,7 @@ struct gdv_arrow_batch_s {
   ArrowDeviceArray array;  // moved from the producer's struct
   SchemaPtr schema;
   std::vector<gdv_column_t> columns;
+  std::vector<gdv_dictionary_t> dictionaries;  // dictionary columns' var_data points here
   gdv_batch_t view;
   int device = -1;  // CUDA ordinal, -1 for host memory
 };
@@ -181,10 +182,22 @@ gdv_status gdv_schema_from_arrow(const struct ArrowSchema* schema, gdv_schema_t*
   for (int64_t i = 0; i < schema->n_children; ++i) {
     const ArrowSchema* c = schema->children[i];
     if (c == nullptr) return Fail(GDV_INVALID, "null child schema");
-    if (c->dictionary != nullptr) return Fail(GDV_NOT_IMPLEMENTED, "dictionary-encoded columns are not supported");
     DataType t;
     Status s = ParseFormat(c->format, &t);
     if (!s.ok()) return Fail(s);
+    if (c->dictionary != nullptr) {
+      // dictionary-encoded: the child's format is the index type's, the dictionary's the values'
+      DataType v;
+      s = ParseFormat(c->dictionary->format, &v);
+      if (s.ok() && (!v.is_varlen() || !t.is_signed_integer()))
+        s = Status::Make(GDV_NOT_IMPLEMENTED, "column '" + std::string(c->name ? c->name : "") +
+                                                  "': dictionaries need utf8 or binary values and signed int8 / int16 / "
+                                                  "int32 / int64 indices");
+      if (!s.ok()) return Fail(s);
+      v.index = t.id;
+      v.ordered = (c->flags & ARROW_FLAG_DICTIONARY_ORDERED) != 0;
+      t = v;
+    }
     fields.push_back(Field{std::string(c->name ? c->name : ""), t});
   }
   *out = reinterpret_cast<gdv_schema_t>(new SchemaH{std::make_shared<Schema>(std::move(fields))});
@@ -214,13 +227,17 @@ gdv_status gdv_arrow_batch_import(struct ArrowDeviceArray* array, gdv_schema_t s
   std::unique_ptr<gdv_arrow_batch_s> b(new gdv_arrow_batch_s());
   b->schema = sch;
   b->device = mem == GDV_MEM_DEVICE ? static_cast<int>(array->device_id) : -1;
+  b->dictionaries.assign(fields.size(), gdv_dictionary_t{});
   for (size_t i = 0; i < fields.size(); ++i) {
     const ArrowArray* c = a.children[i];
     const DataType& t = fields[i].type;
     if (c == nullptr) return Fail(GDV_INVALID, "null child array");
-    if (c->dictionary != nullptr || c->n_children != 0)
-      return Fail(GDV_NOT_IMPLEMENTED, "nested / dictionary columns are not supported");
-    const int64_t want = t.is_varlen() ? 3 : 2;
+    if (c->n_children != 0) return Fail(GDV_NOT_IMPLEMENTED, "nested columns are not supported");
+    if ((c->dictionary != nullptr) != t.is_dict())
+      return Fail(c->dictionary != nullptr ? GDV_NOT_IMPLEMENTED : GDV_INVALID,
+                  "column '" + fields[i].name + "': the array " + (c->dictionary != nullptr ? "is" : "is not") +
+                      " dictionary-encoded but the schema's type is " + t.ToString());
+    const int64_t want = t.is_varlen() && !t.is_dict() ? 3 : 2;
     if (c->n_buffers != want)
       return Fail(GDV_INVALID, "column '" + fields[i].name + "': expected " + std::to_string(want) +
                                    " buffers, got " + std::to_string(c->n_buffers));
@@ -231,7 +248,23 @@ gdv_status gdv_arrow_batch_import(struct ArrowDeviceArray* array, gdv_schema_t s
     col.validity = c->null_count == 0 ? nullptr : c->buffers[0];
     col.values = c->buffers[1];
     col.offset = c->offset + a.offset;
-    if (t.is_varlen()) {
+    if (t.is_dict()) {
+      // zero copy: the dictionary's buffers are read where the producer put them
+      const ArrowArray* d = c->dictionary;
+      if (d->n_buffers != 3 || d->n_children != 0 || d->dictionary != nullptr || d->length < 0 || d->offset < 0 ||
+          (d->length > 0 && d->buffers[1] == nullptr))
+        return Fail(GDV_INVALID, "column '" + fields[i].name + "': malformed dictionary (expected a utf8 / binary "
+                                 "array of 3 buffers with offsets)");
+      gdv_dictionary_t& dict = b->dictionaries[i];
+      dict.validity = d->null_count == 0 ? nullptr : d->buffers[0];
+      dict.offsets = d->buffers[1];
+      dict.data = d->buffers[2];
+      dict.offset = d->offset;
+      dict.length = d->length;
+      if (mem == GDV_MEM_HOST && d->length > 0)
+        dict.data_size = static_cast<const int32_t*>(d->buffers[1])[d->offset + d->length];
+      col.var_data = &dict;
+    } else if (t.is_varlen()) {
       col.var_data = c->buffers[2];
       if (mem == GDV_MEM_HOST && c->buffers[1] != nullptr)
         col.var_data_size = static_cast<const int32_t*>(c->buffers[1])[col.offset + a.length];

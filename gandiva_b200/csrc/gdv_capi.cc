@@ -390,6 +390,10 @@ gdv_status gdv_filter_kernel_info(gdv_filter_t f, char* name_buf, int64_t name_l
 gdv_status gdv_filter_kernel_attr(gdv_filter_t f, const char* key, int64_t* out) {
   if (f == nullptr) return Fail(GDV_INVALID, "null filter");
   auto& fl = *reinterpret_cast<FiltH*>(f)->p;
+  if (key != nullptr && out != nullptr && std::string(key) == "dictionary_first") {
+    *out = fl.dictionary_first_used() ? 1 : 0;
+    return GDV_OK;
+  }
   CompiledKernel* k = fl.last_used();
   if (k == nullptr) {
     Status s = fl.KernelFor(GDV_SEL_UINT32, true, false, &k);

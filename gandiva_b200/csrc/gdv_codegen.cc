@@ -19,6 +19,12 @@ namespace {
 
 Status VErr(const std::string& m) { return Status::Make(GDV_EXPRESSION_VALIDATION_ERROR, m); }
 
+// Dictionary-encoded columns are inputs only: results are plain utf8 / binary, as Gandiva's are.
+Status DictionaryResult(const std::string& what) {
+  return Status::Make(GDV_NOT_IMPLEMENTED, "'" + what + "' has a dictionary result type: dictionary-encoded "
+                                           "outputs are not supported (results are plain utf8 / binary)");
+}
+
 bool IsSupportedType(const DataType& t) {
   switch (t.id) {
     case GDV_TYPE_BOOL: case GDV_TYPE_UINT8: case GDV_TYPE_INT8: case GDV_TYPE_UINT16:
@@ -54,23 +60,33 @@ Status ValidateNode(const Schema& schema, const Node& node) {
       const auto& f = static_cast<const FieldNode&>(node);
       const int idx = schema.index_of(f.name());
       if (idx < 0) return VErr("Field " + f.name() + " not in schema");
-      if (schema.fields()[idx].type != f.return_type())
+      if (!schema.fields()[idx].type.same(f.return_type()))
         return VErr("Field definition in schema " + schema.fields()[idx].name + ": " +
                     schema.fields()[idx].type.ToString() +
                     " different from field in expression " + f.ToString());
+      if (f.return_type().is_dict()) {
+        const DataType& t = f.return_type();
+        if (!t.is_varlen() || !DataType(t.index).is_signed_integer())
+          return Status::Make(GDV_NOT_IMPLEMENTED,
+                              "Field " + f.name() + " has unsupported data type " + t.ToString() +
+                                  ": dictionary columns need utf8 or binary values and int8, int16, "
+                                  "int32 or int64 indices");
+        return Status::OK();
+      }
       if (!IsSupportedType(f.return_type()))
         return VErr("Field " + f.name() + " has unsupported data type " +
                     f.return_type().ToString());
       return Status::OK();
     }
     case NodeKind::kLiteral: {
-      if (!IsSupportedType(node.return_type()))
+      if (!IsSupportedType(node.return_type()) || node.return_type().is_dict())
         return VErr("Value " + node.ToString() + " has unsupported data type " +
                     node.return_type().ToString());
       return Status::OK();
     }
     case NodeKind::kFunction: {
       const auto& fn = static_cast<const FunctionNode&>(node);
+      if (fn.return_type().is_dict()) return DictionaryResult(fn.name());
       std::vector<DataType> params;
       for (const auto& c : fn.children()) {
         Status s = ValidateNode(schema, *c);
@@ -150,6 +166,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
     }
     case NodeKind::kIf: {
       const auto& n = static_cast<const IfNode&>(node);
+      if (n.return_type().is_dict()) return DictionaryResult("if");
       for (const NodePtr* c : {&n.condition(), &n.then_node(), &n.else_node()}) {
         Status s = ValidateNode(schema, **c);
         if (!s.ok()) return s;
@@ -203,6 +220,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
 
 Status ValidateExpression(const Schema& schema, const Expression& expr) {
   if (expr.root() == nullptr) return VErr("Expression has no root node");
+  if (expr.result().type.is_dict()) return DictionaryResult(expr.result().name);
   Status s = ValidateNode(schema, *expr.root());
   if (!s.ok()) return s;
   if (expr.root()->return_type() != expr.result().type)
@@ -214,8 +232,8 @@ Status ValidateExpression(const Schema& schema, const Expression& expr) {
 // ======================================================================================
 // Args layout
 // ======================================================================================
-ArgsLayout::ArgsLayout(int n_inputs, int n_outputs)
-    : ni(std::max(n_inputs, 1)), no(std::max(n_outputs, 1)) {
+ArgsLayout::ArgsLayout(int n_inputs, int n_outputs, bool dictionary)
+    : ni(std::max(n_inputs, 1)), no(std::max(n_outputs, 1)), dict(dictionary) {
   size_t o = 80;
   off_in_val = o; o += 8u * ni;
   off_in_vld = o; o += 8u * ni;
@@ -225,7 +243,20 @@ ArgsLayout::ArgsLayout(int n_inputs, int n_outputs)
   off_out_var = o; o += 8u * no;
   off_in_vsh = o; o += 4u * ni;
   off_in_dsh = o; o += 4u * ni;
+  if (dict) {
+    o = (o + 7u) & ~size_t(7);
+    off_in_dof = o; o += 8u * ni;
+    off_in_dvl = o; o += 8u * ni;
+    off_in_dln = o; o += 8u * ni;
+    off_in_dvs = o; o += 4u * ni;
+  }
   size = (o + 7u) & ~size_t(7);
+}
+
+bool HasDictionary(const std::vector<ColumnSlot>& slots) {
+  for (const auto& s : slots)
+    if (s.type.is_dict()) return true;
+  return false;
 }
 
 // ======================================================================================
@@ -569,7 +600,7 @@ class BodyGen {
   Val GenField(const FieldNode& f) {
     const int j = SlotFor(f);
     return Val{"f" + std::to_string(j) + "[k]",
-               nullable_ ? "k" + std::to_string(j) + "[k]" : std::string("true"), f.return_type()};
+               nullable_ ? "k" + std::to_string(j) + "[k]" : std::string("true"), f.return_type().value_type()};
   }
 
   std::string BytesArray(const std::string& bytes, const char* prefix) {
@@ -683,7 +714,8 @@ class BodyGen {
   // which is what the cooperative LIKE scan needs.
   bool ViewChain(const Node& node, int* slot, unsigned* xf) {
     if (node.kind() == NodeKind::kField) {
-      if (!node.return_type().is_varlen()) return false;
+      // a dictionary column's rows are not one contiguous run of bytes
+      if (!node.return_type().is_varlen() || node.return_type().is_dict()) return false;
       *slot = SlotFor(static_cast<const FieldNode&>(node));
       *xf = 0u;
       return true;
@@ -1340,8 +1372,13 @@ std::string EmitArgsStruct(const ArgsLayout& L) {
     << "  u32* out_vld[" << L.no << "];\n"
     << "  u8* out_var[" << L.no << "];\n"
     << "  u32 in_vsh[" << L.ni << "];\n"
-    << "  u32 in_dsh[" << L.ni << "];\n"
-    << "};\n";
+    << "  u32 in_dsh[" << L.ni << "];\n";
+  if (L.dict)
+    s << "  const i32* in_dof[" << L.ni << "];  // dictionary columns: the dictionary's offsets,\n"
+      << "  const u32* in_dvl[" << L.ni << "];  // validity words (or null),\n"
+      << "  i64 in_dln[" << L.ni << "];         // length\n"
+      << "  u32 in_dvs[" << L.ni << "];         // and validity bit shift; in_var = its bytes\n";
+  s << "};\n";
   return s.str();
 }
 
@@ -1363,6 +1400,14 @@ void EmitPrologue(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, 
     if (t.is_bool()) {
       *o += "  const u32* in_dat" + J + " = reinterpret_cast<const u32*>(A.in_val[" + J + "]);\n";
       *o += "  const u32 in_dsh" + J + " = A.in_dsh[" + J + "];\n";
+    } else if (t.is_dict()) {
+      const std::string it = DataType(t.index).ctype();
+      *o += "  const " + it + "* in_val" + J + " = reinterpret_cast<const " + it + "*>(A.in_val[" + J + "]);\n";
+      *o += "  const u8* in_var" + J + " = A.in_var[" + J + "];\n";
+      *o += "  const i32* in_dof" + J + " = A.in_dof[" + J + "];\n";
+      *o += "  const u32* in_dvl" + J + " = A.in_dvl[" + J + "];\n";
+      *o += "  const i64 in_dln" + J + " = A.in_dln[" + J + "];\n";
+      *o += "  const u32 in_dvs" + J + " = A.in_dvs[" + J + "];\n";
     } else if (t.is_varlen()) {
       *o += "  const i32* in_val" + J + " = reinterpret_cast<const i32*>(A.in_val[" + J + "]);\n";
       *o += "  const u8* in_var" + J + " = A.in_var[" + J + "];\n";
@@ -1540,6 +1585,17 @@ std::string EmitCoopScan(int j, const std::vector<CoopSeg>& segs, int R, const s
   return o;
 }
 
+// Row view of dictionary column J for the index expression `ix` (gdv_dict_view); the entry's
+// validity lands in d<J>[k].
+std::string DictView(const std::string& J, const std::string& ix) {
+  return "gdv_dict_view(in_dof" + J + ", in_var" + J + ", in_dvl" + J + ", in_dvs" + J + ", in_dln" + J + ", " + ix +
+         ", &d" + J + "[k])";
+}
+
+// A utf8 / binary column whose group of rows is one contiguous run of the data buffer (what the
+// shared-memory string stage copies); a dictionary column's rows are not.
+bool HasByteRun(const ColumnSlot& s) { return s.type.is_varlen() && !s.type.is_dict(); }
+
 bool SlotHasCoop(const std::vector<CoopSeg>& segs, int j) {
   for (const auto& cs : segs)
     if (cs.slot == j) return true;
@@ -1558,7 +1614,10 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
     const DataType& t = slots[j].type;
     *o += I + t.ctype() + " f" + std::to_string(j) + "[" + sR + "];\n";
     if (spec.nullable) *o += I + "bool k" + std::to_string(j) + "[" + sR + "];\n";
-    if (t.is_varlen()) {
+    if (t.is_dict()) {
+      // dictionary column: the entry behind the row's index is valid (and the index in range)
+      *o += I + "bool d" + std::to_string(j) + "[" + sR + "];\n";
+    } else if (t.is_varlen()) {
       // group state of the string stage: rows known to be ASCII, cooperative-scan hit list usable
       *o += I + "u32 ascii" + std::to_string(j) + " = 0u;\n";
       if (SlotHasCoop(coop, static_cast<int>(j))) {
@@ -1587,9 +1646,11 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
       const DataType& t = slots[j].type;
       const std::string J = std::to_string(j);
       if (!t.is_bool())
-        *o += I + "const " + (t.is_varlen() ? std::string("i32") : std::string(t.ctype())) +
+        *o += I + "const " +
+              (t.is_dict() ? std::string(DataType(t.index).ctype())
+                           : t.is_varlen() ? std::string("i32") : std::string(t.ctype())) +
               "* ptr" + J + " = in_val" + J + " + base + (i64)lane;\n";
-      if (t.is_varlen() && stage_bytes > 0) {
+      if (t.is_varlen() && !t.is_dict() && stage_bytes > 0) {
         // The bytes of the group's 32*R strings are one contiguous run: copy it into this
         // warp's shared-memory stage with coalesced 16-byte loads, then every lane walks its
         // own string out of shared memory instead of issuing one global load per byte.
@@ -1647,6 +1708,8 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
       if (t.is_bool()) {
         *o += I + "  f" + J + "[k] = ((gdv_ldwin(in_dat" + J + ", (base >> 5) + k, in_dsh" + J +
               ") >> lane) & 1u) != 0u;\n";
+      } else if (t.is_dict()) {
+        *o += I + "  f" + J + "[k] = " + DictView(J, "(i64)gdv_ldp(ptr" + J + " + 32 * k)") + ";\n";
       } else if (t.is_varlen()) {
         *o += I + "  { const i32 sb = ptr" + J + "[32 * k]; const i32 se = ptr" + J +
               "[32 * k + 1]; f" + J + "[k] = gdv_make_str(" +
@@ -1666,7 +1729,7 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
           *o += I + "  k" + J + "[k] = true;\n";
         else
           *o += I + "  k" + J + "[k] = ((gdv_ldwin(in_vp" + J + ", ((base >> 5) + k) & in_vm" + J + ", in_vsh" +
-                J + ") >> lane) & 1u) != 0u;\n";
+                J + ") >> lane) & 1u) != 0u" + (slots[j].type.is_dict() ? " && d" + J + "[k]" : "") + ";\n";
       }
       *o += I + "}\n";
     }
@@ -1682,6 +1745,8 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
       if (t.is_bool()) {
         *o += I + "  f" + J + "[k] = in && gdv_ldbit(reinterpret_cast<const u8*>(in_dat" + J + "), in_dsh" +
               J + ", r);\n";
+      } else if (t.is_dict()) {
+        *o += I + "  f" + J + "[k] = " + DictView(J, "in ? (i64)gdv_ldp(in_val" + J + " + r) : -1ll") + ";\n";
       } else if (t.is_varlen()) {
         *o += I + "  { const i32 sb = in ? in_val" + J + "[r] : 0; const i32 se = in ? in_val" + J +
               "[r + 1] : 0; f" + J + "[k] = gdv_make_str(in_var" + J + " + sb, se - sb); }\n";
@@ -1692,7 +1757,7 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
         *o += I + "  k" + J + "[k] = in;\n";
       else if (spec.nullable)
         *o += I + "  k" + J + "[k] = in && (!in_hv" + J + " || gdv_ldbit(reinterpret_cast<const u8*>(in_vld" +
-              J + "), in_vsh" + J + ", r));\n";
+              J + "), in_vsh" + J + ", r))" + (t.is_dict() ? " && d" + J + "[k]" : "") + ";\n";
     }
     *o += I + "}\n";
   }
@@ -2153,8 +2218,9 @@ void ApplyDeviceCount(std::string* src) {
 void MarkHoisted(const BodyGen& gen, const Node& cond, std::vector<ColumnSlot>* slots) {
   std::vector<int> strict;
   gen.TruthStrict(cond, &strict);
-  for (auto& sl : *slots)
-    if (std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end()) sl.hoist = true;
+  for (auto& sl : *slots)  // a dictionary row's validity also depends on its entry: read per row
+    if (!sl.type.is_dict() && std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end())
+      sl.hoist = true;
 }
 
 int PickRowsPerThread(int in_bytes, int out_bytes, KernelKind kind) {
@@ -2189,7 +2255,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
   int n_varlen = 0, in_bytes = 0;
   for (const auto& s : slots) {
-    n_varlen += s.type.is_varlen() ? 1 : 0;
+    n_varlen += HasByteRun(s) ? 1 : 0;
     in_bytes += s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);
   }
   int R = spec.rows_per_thread > 0 ? std::min(spec.rows_per_thread, 8) : 2;
@@ -2216,7 +2282,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   const int col_block = stage_bytes + hit_bytes;
   const int dynamic_smem = col_block * NW * n_varlen;
   const bool has_sel = spec.selection_mode != GDV_SEL_NONE;
-  ArgsLayout L(static_cast<int>(slots.size()), 1);
+  ArgsLayout L(static_cast<int>(slots.size()), 1, HasDictionary(slots));
   const std::string sR = std::to_string(R), s32R = std::to_string(32 * R), sT = std::to_string(T);
 
   std::string src;
@@ -2241,7 +2307,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
     src += "  extern __shared__ uint4 gdv_smem[];\n";
     int vi = 0;
     for (size_t j = 0; j < slots.size(); ++j) {
-      if (!slots[j].type.is_varlen()) continue;
+      if (!HasByteRun(slots[j])) continue;
       const std::string J = std::to_string(j);
       src += "  u8* stage" + J + " = reinterpret_cast<u8*>(gdv_smem) + ((size_t)wid * " +
              std::to_string(n_varlen) + " + " + std::to_string(vi) + ") * " + std::to_string(col_block) + ";\n";
@@ -2478,14 +2544,109 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
 
 }  // namespace
 
+namespace {
+void CollectColumns(const Schema& schema, const Node& node, std::vector<int>* cols) {
+  switch (node.kind()) {
+    case NodeKind::kField: {
+      const int i = schema.index_of(static_cast<const FieldNode&>(node).name());
+      if (std::find(cols->begin(), cols->end(), i) == cols->end()) cols->push_back(i);
+      return;
+    }
+    case NodeKind::kLiteral: return;
+    case NodeKind::kFunction:
+      for (const auto& c : static_cast<const FunctionNode&>(node).children()) CollectColumns(schema, *c, cols);
+      return;
+    case NodeKind::kIf: {
+      const auto& n = static_cast<const IfNode&>(node);
+      for (const NodePtr* c : {&n.condition(), &n.then_node(), &n.else_node()}) CollectColumns(schema, **c, cols);
+      return;
+    }
+    case NodeKind::kBoolean:
+      for (const auto& c : static_cast<const BooleanNode&>(node).children()) CollectColumns(schema, *c, cols);
+      return;
+    case NodeKind::kIn: CollectColumns(schema, *static_cast<const InNode&>(node).child(), cols); return;
+  }
+}
+}  // namespace
+
+int DictionaryFirstColumn(const Schema& schema, const Node& cond) {
+  std::vector<int> cols;
+  CollectColumns(schema, cond, &cols);
+  if (cols.size() != 1 || cols[0] < 0 || !schema.fields()[cols[0]].type.is_dict()) return -1;
+  if (BodyGen::CanFail(cond)) return -1;  // errors must come from the rows that hold the value
+  std::vector<ColumnSlot> slots;
+  const BodyGen gen(schema, &slots, true, false);
+  std::vector<int> strict;
+  gen.TruthStrict(cond, &strict);
+  return std::find(strict.begin(), strict.end(), cols[0]) != strict.end() ? cols[0] : -1;
+}
+
+NodePtr WithValueTypes(const NodePtr& node) {
+  switch (node->kind()) {
+    case NodeKind::kField: {
+      const auto& f = static_cast<const FieldNode&>(*node);
+      if (!f.return_type().is_dict()) return node;
+      return std::make_shared<FieldNode>(f.name(), f.return_type().value_type());
+    }
+    case NodeKind::kLiteral: return node;
+    case NodeKind::kFunction: {
+      const auto& fn = static_cast<const FunctionNode&>(*node);
+      NodeVector kids;
+      for (const auto& c : fn.children()) kids.push_back(WithValueTypes(c));
+      return std::make_shared<FunctionNode>(fn.name(), std::move(kids), fn.return_type());
+    }
+    case NodeKind::kIf: {
+      const auto& n = static_cast<const IfNode&>(*node);
+      return std::make_shared<IfNode>(WithValueTypes(n.condition()), WithValueTypes(n.then_node()),
+                                      WithValueTypes(n.else_node()), n.return_type());
+    }
+    case NodeKind::kBoolean: {
+      const auto& n = static_cast<const BooleanNode&>(*node);
+      NodeVector kids;
+      for (const auto& c : n.children()) kids.push_back(WithValueTypes(c));
+      return std::make_shared<BooleanNode>(n.op(), std::move(kids));
+    }
+    case NodeKind::kIn: {
+      const auto& n = static_cast<const InNode&>(*node);
+      return std::make_shared<InNode>(WithValueTypes(n.child()), n.value_type(), n.ints(), n.strs());
+    }
+  }
+  return node;
+}
+
+static bool ReadsDictionary(const Node& node) {
+  switch (node.kind()) {
+    case NodeKind::kField: return node.return_type().is_dict();
+    case NodeKind::kLiteral: return false;
+    case NodeKind::kFunction:
+      for (const auto& c : static_cast<const FunctionNode&>(node).children())
+        if (ReadsDictionary(*c)) return true;
+      return false;
+    case NodeKind::kIf: {
+      const auto& n = static_cast<const IfNode&>(node);
+      return ReadsDictionary(*n.condition()) || ReadsDictionary(*n.then_node()) || ReadsDictionary(*n.else_node());
+    }
+    case NodeKind::kBoolean:
+      for (const auto& c : static_cast<const BooleanNode&>(node).children())
+        if (ReadsDictionary(*c)) return true;
+      return false;
+    case NodeKind::kIn: return ReadsDictionary(*static_cast<const InNode&>(node).child());
+  }
+  return false;
+}
+
 Status GenerateKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs,
                       const KernelSpec& spec, GeneratedKernel* out) {
   std::vector<ExpressionPtr> lowered;
+  KernelSpec s = spec;
   for (const auto& e : exprs) {
     NodePtr r = RewriteAliases(e->root());
     lowered.push_back(r == e->root() ? e : std::make_shared<Expression>(r, e->result()));
+    // a dictionary row is null when its entry is, or when its index is out of range: such kernels
+    // always keep the validity plumbing
+    if (ReadsDictionary(*r)) s.nullable = true;
   }
-  return GenerateKernelImpl(schema, lowered, spec, out);
+  return GenerateKernelImpl(schema, lowered, s, out);
 }
 
 namespace {
@@ -2512,7 +2673,8 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     if (kBT % 32 == 0 && kBT <= 1024 && kgen.PlanKey(*exprs[0]->root(), &plan)) {
       std::string kbody;
       const Val kres = kgen.GenTruth(*exprs[0]->root(), &kbody, 6);
-      if (kgen.error().empty() && !kgen.uses_ctx()) {
+      // the anchor drain loads rows one by one from plain columns only
+      if (kgen.error().empty() && !kgen.uses_ctx() && !HasDictionary(kslots)) {
         if (spec.nullable) MarkHoisted(kgen, *exprs[0]->root(), &kslots);
         ArgsLayout KL(static_cast<int>(kslots.size()), 0);
         std::string src = "// generated by gandiva_b200 kernel fuser; key-driven string Filter";
@@ -2570,8 +2732,9 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   int in_bytes = 0, out_bytes = 0;
   int n_varlen = 0;
   for (const auto& s : slots) {
-    in_bytes += s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);  // 4 B offset + ~28 B data
-    n_varlen += s.type.is_varlen() ? 1 : 0;
+    in_bytes += s.type.is_dict() ? DataType(s.type.index).width()  // the index; the dictionary is cached
+                : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);  // 4 B offset + ~28 B data
+    n_varlen += HasByteRun(s) ? 1 : 0;
   }
   for (const auto& e : exprs) out_bytes += std::max(e->result().type.width(), 1);
   if (spec.kind == KernelKind::kFilter) out_bytes = 0;
@@ -2658,7 +2821,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
       dynamic_smem = S * stage_total;
     }
   }
-  ArgsLayout L(static_cast<int>(slots.size()), n_out);
+  ArgsLayout L(static_cast<int>(slots.size()), n_out, HasDictionary(slots));
 
   std::string src;
   src += "// generated by gandiva_b200 kernel fuser; one fused kernel per ";
@@ -2676,7 +2839,8 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   std::string bounds = sBT;
   bool light = spec.kind == KernelKind::kFilter && n_varlen == 0 && BT >= 256 && 2048 % BT == 0 &&
                !gen.uses_ctx() && body.size() < 6000;
-  for (const auto& sl : slots) light = light && !sl.type.is_decimal();  // 128-bit math wants registers
+  for (const auto& sl : slots)  // 128-bit math and string functions over dictionary views want registers
+    light = light && !sl.type.is_decimal() && !sl.type.is_dict();
   if (W > 1) light = false;  // W chunks keep 2 W more registers
   if (light) bounds += ", " + std::to_string(2048 / BT);
   src += "extern \"C\" __global__ void __launch_bounds__(" + bounds + ") " + spec.name +
@@ -2690,7 +2854,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     src += "  extern __shared__ uint4 gdv_smem[];\n";
     int vi = 0;
     for (size_t j = 0; j < slots.size(); ++j) {
-      if (!slots[j].type.is_varlen()) continue;
+      if (!HasByteRun(slots[j])) continue;
       const std::string SJ = "stage" + std::to_string(j) + (prefetch ? "_0" : "");
       src += "  u8* const " + SJ + " = reinterpret_cast<u8*>(gdv_smem) + ((size_t)wid * " +
              std::to_string(n_varlen) + " + " + std::to_string(vi) + ") * " +
@@ -2911,7 +3075,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
       // issue(b, par): cp.async the bytes of the full group that starts at row b into stage `par`
       src += "    auto issue = [&](i64 b, u32 par) {\n";
       for (size_t j = 0; j < slots.size(); ++j) {
-        if (!slots[j].type.is_varlen()) continue;
+        if (!HasByteRun(slots[j])) continue;
         const std::string J = std::to_string(j);
         src += "      {\n";
         src += "        const i32 gb = in_val" + J + "[b];\n";
@@ -2935,7 +3099,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
       src += "      const i64 base = wbase + 32 * g;\n";
       src += "      if (base >= A.n) break;\n";
       for (size_t j = 0; j < slots.size(); ++j)
-        if (slots[j].type.is_varlen())
+        if (HasByteRun(slots[j]))
           src += "      u8* const stage" + std::to_string(j) + " = stage" + std::to_string(j) +
                  "_0 + (size_t)par * " + std::to_string(stage_bytes) + "u;\n";
       src += "      if (base + " + s32R + " <= A.n) {\n";

@@ -86,10 +86,24 @@ struct ArgsLayout {
          off_tile_state = 40, off_ticket = 48, off_err = 56, off_out_cap = 64, off_n_ptr = 72;
   size_t off_in_val, off_in_vld, off_in_var, off_out_val, off_out_vld, off_out_var, off_in_vsh,
       off_in_dsh, size;
-  ArgsLayout(int n_inputs, int n_outputs);
+  // Kernels that read a dictionary column get one more block per input (HasDictionary): the
+  // dictionary's offsets, validity word pointer, length and validity bit shift.  Zero otherwise.
+  bool dict = false;
+  size_t off_in_dof = 0, off_in_dvl = 0, off_in_dln = 0, off_in_dvs = 0;
+  ArgsLayout(int n_inputs, int n_outputs, bool dictionary = false);
 };
+
+bool HasDictionary(const std::vector<ColumnSlot>& slots);
 
 Status GenerateKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs,
                       const KernelSpec& spec, GeneratedKernel* out);
+
+// Filter conditions that can be evaluated once per dictionary entry (DESIGN.md §3.6): the condition
+// reads exactly one column, that column is dictionary-encoded, nothing in it can raise, and a null in
+// the column makes it not-true (so a null index, a null entry or an index out of range is never kept).
+// Returns the column's schema index, or -1.
+int DictionaryFirstColumn(const Schema& schema, const Node& cond);
+// The same tree with every dictionary-encoded field read as a plain column of its value type.
+NodePtr WithValueTypes(const NodePtr& node);
 
 }  // namespace gdv

@@ -30,6 +30,9 @@ static const char* unit_name(int u) {
 }
 
 std::string DataType::ToString() const {
+  if (index != 0)
+    return "dictionary<values=" + value_type().ToString() + ", indices=" + DataType(index).ToString() +
+           ", ordered=" + (ordered ? "1" : "0") + ">";
   switch (id) {
     case GDV_TYPE_NA: return "null";
     case GDV_TYPE_BOOL: return "bool";

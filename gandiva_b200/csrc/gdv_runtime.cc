@@ -424,15 +424,71 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
   return Status::OK();
 }
 
-// One kernel input after staging: device addresses + bit shifts.
+// One kernel input after staging: device addresses + bit shifts.  Dictionary columns: val / vld /
+// vsh are the indices', var the dictionary's bytes, and dof / dvl / dvs / dln the dictionary's
+// offsets, validity words, bit shift and length.
 struct ResolvedIn {
   CUdeviceptr val = 0, vld = 0, var = 0;
   uint32_t vsh = 0, dsh = 0;
+  CUdeviceptr dof = 0, dvl = 0;
+  uint32_t dvs = 0;
+  int64_t dln = 0;
 };
 
 inline int64_t BitBytes(int64_t bit_begin, int64_t nbits) {
   // bytes that cover bits [bit_begin, bit_begin + nbits) counted from the byte of bit_begin
   return ((bit_begin & 7) + nbits + 7) / 8;
+}
+
+// A bitmap of `nbits` bits from bit `off` on as the kernels read it: a 4-byte aligned word pointer
+// plus a bit shift in [0, 31] (host bitmaps are staged into pooled device memory first).
+Status ResolveBitmap(Device* dev, const void* bits, int64_t off, int64_t nbits, bool host, CUstream stream,
+                     ScratchScope* scratch, CUdeviceptr* ptr, uint32_t* sh) {
+  const uint8_t* p = static_cast<const uint8_t*>(bits) + (off >> 3);
+  *sh = static_cast<uint32_t>(off & 7);
+  if (host) {
+    const size_t bytes = static_cast<size_t>(BitBytes(off, nbits));
+    GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 8, ptr));
+    if (bytes > 0) GDV_RETURN_NOT_OK(StagedHtoD(dev, *ptr, p, bytes, stream));
+  } else {
+    const uintptr_t mis = reinterpret_cast<uintptr_t>(p) & 3u;
+    *ptr = reinterpret_cast<CUdeviceptr>(p - mis);
+    *sh += static_cast<uint32_t>(8 * mis);
+  }
+  return Status::OK();
+}
+
+// The dictionary of a dictionary-encoded column (gdv_dictionary_t, reached through var_data).
+Status ResolveDictionary(Device* dev, int col, const gdv_column_t& c, bool host, CUstream stream,
+                         ScratchScope* scratch, ResolvedIn* r) {
+  const auto* dict = static_cast<const gdv_dictionary_t*>(c.var_data);
+  const std::string what = "dictionary column " + std::to_string(col);
+  if (dict == nullptr) return Status::Make(GDV_INVALID, what + " has no dictionary (var_data must point at a gdv_dictionary_t)");
+  if (dict->length < 0 || dict->offset < 0) return Status::Make(GDV_INVALID, what + ": negative dictionary length or offset");
+  r->dln = dict->length;
+  if (dict->length == 0) return Status::OK();  // every index is out of range: no row reads it
+  if (dict->offsets == nullptr) return Status::Make(GDV_INVALID, what + ": the dictionary has no offsets buffer");
+  const int32_t* offs = static_cast<const int32_t*>(dict->offsets) + dict->offset;
+  if (dict->validity != nullptr)
+    GDV_RETURN_NOT_OK(ResolveBitmap(dev, dict->validity, dict->offset, dict->length, host, stream, scratch, &r->dvl, &r->dvs));
+  if (!host) {
+    r->dof = reinterpret_cast<CUdeviceptr>(offs);
+    r->var = reinterpret_cast<CUdeviceptr>(dict->data);
+    return Status::OK();
+  }
+  const size_t obytes = static_cast<size_t>(dict->length + 1) * 4;
+  GDV_RETURN_NOT_OK(scratch->Alloc(obytes, &r->dof));
+  GDV_RETURN_NOT_OK(StagedHtoD(dev, r->dof, offs, obytes, stream));
+  const int64_t first = offs[0], last = offs[dict->length];
+  if (first < 0 || last < first || (last > first && (dict->data == nullptr || last > dict->data_size)))
+    return Status::Make(GDV_INVALID, what + ": the dictionary's offsets reach past its data buffer");
+  const size_t vbytes = static_cast<size_t>(last - first);
+  CUdeviceptr dv;
+  GDV_RETURN_NOT_OK(scratch->Alloc(vbytes + 16, &dv));
+  if (vbytes > 0)
+    GDV_RETURN_NOT_OK(StagedHtoD(dev, dv, static_cast<const uint8_t*>(dict->data) + first, vbytes, stream));
+  r->var = dv - static_cast<CUdeviceptr>(first);  // kernel addresses bytes as var + offs[i]
+  return Status::OK();
 }
 
 Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t* batch,
@@ -483,6 +539,23 @@ Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t*
         r.val = reinterpret_cast<CUdeviceptr>(p - mis);
         r.dsh += static_cast<uint32_t>(8 * mis);
       }
+    } else if (t.is_dict()) {
+      // the indices like a fixed-width column of the index type, then the dictionary
+      const int w = DataType(t.index).width();
+      const uint8_t* p = static_cast<const uint8_t*>(c.values) + off * w;
+      if (host) {
+        const size_t bytes = static_cast<size_t>(n) * w;
+        CUdeviceptr dp;
+        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 16, &dp));
+        if (bytes > 0) GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
+        r.val = dp;
+      } else {
+        if (reinterpret_cast<uintptr_t>(p) % static_cast<uintptr_t>(w) != 0)
+          return Status::Make(GDV_INVALID, "device indices buffer of column " + std::to_string(slot.schema_index) +
+                                               " is not aligned to its element width");
+        r.val = reinterpret_cast<CUdeviceptr>(p);
+      }
+      GDV_RETURN_NOT_OK(ResolveDictionary(dev, slot.schema_index, c, host, stream, scratch, &r));
     } else if (t.is_varlen()) {
       const int32_t* offs = static_cast<const int32_t*>(c.values) + off;
       if (host) {
@@ -529,6 +602,22 @@ Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t*
 template <typename T>
 void Put(std::vector<uint8_t>& buf, size_t off, T v) {
   std::memcpy(buf.data() + off, &v, sizeof(T));
+}
+
+void PutInputs(std::vector<uint8_t>& args, const ArgsLayout& L, const std::vector<ResolvedIn>& ins) {
+  for (size_t j = 0; j < ins.size(); ++j) {
+    Put<CUdeviceptr>(args, L.off_in_val + 8 * j, ins[j].val);
+    Put<CUdeviceptr>(args, L.off_in_vld + 8 * j, ins[j].vld);
+    Put<CUdeviceptr>(args, L.off_in_var + 8 * j, ins[j].var);
+    Put<uint32_t>(args, L.off_in_vsh + 4 * j, ins[j].vsh);
+    Put<uint32_t>(args, L.off_in_dsh + 4 * j, ins[j].dsh);
+    if (L.dict) {
+      Put<CUdeviceptr>(args, L.off_in_dof + 8 * j, ins[j].dof);
+      Put<CUdeviceptr>(args, L.off_in_dvl + 8 * j, ins[j].dvl);
+      Put<int64_t>(args, L.off_in_dln + 8 * j, ins[j].dln);
+      Put<uint32_t>(args, L.off_in_dvs + 4 * j, ins[j].dvs);
+    }
+  }
 }
 
 Status LaunchKernel(Device* dev, const CompiledKernel::Loaded& l, const GeneratedKernel& gen,
@@ -771,11 +860,12 @@ Status Projector::KernelFor(bool nullable, CompiledKernel** out) {
   return Status::OK();
 }
 
-// True when some column the kernel reads carries a validity bitmap.
+// True when some column the kernel reads carries a validity bitmap, or is dictionary-encoded (a
+// row is also null where its dictionary entry is).
 static bool AnyValidity(const GeneratedKernel& gen, const gdv_batch_t* batch) {
   for (const auto& slot : gen.inputs)
-    if (slot.schema_index >= 0 && slot.schema_index < batch->num_columns &&
-        batch->columns[slot.schema_index].validity != nullptr)
+    if (slot.type.is_dict() || (slot.schema_index >= 0 && slot.schema_index < batch->num_columns &&
+                                batch->columns[slot.schema_index].validity != nullptr))
       return true;
   return false;
 }
@@ -864,16 +954,10 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   scratch.Guard(stream);
   std::vector<ResolvedIn> ins;
   GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), 1);
+  ArgsLayout L(static_cast<int>(gen.inputs.size()), 1, HasDictionary(gen.inputs));
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
-  for (size_t j = 0; j < ins.size(); ++j) {
-    Put<CUdeviceptr>(args, L.off_in_val + 8 * j, ins[j].val);
-    Put<CUdeviceptr>(args, L.off_in_vld + 8 * j, ins[j].vld);
-    Put<CUdeviceptr>(args, L.off_in_var + 8 * j, ins[j].var);
-    Put<uint32_t>(args, L.off_in_vsh + 4 * j, ins[j].vsh);
-    Put<uint32_t>(args, L.off_in_dsh + 4 * j, ins[j].dsh);
-  }
+  PutInputs(args, L, ins);
   if (selection_mode_ != GDV_SEL_NONE) {
     CUdeviceptr dsel = reinterpret_cast<CUdeviceptr>(sel->indices);
     if (host) {
@@ -1028,16 +1112,10 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
   GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
   const double t_inputs = TraceOn() ? NowUs() : 0.0;
 
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), n_outs);
+  ArgsLayout L(static_cast<int>(gen.inputs.size()), n_outs, HasDictionary(gen.inputs));
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
-  for (size_t j = 0; j < ins.size(); ++j) {
-    Put<CUdeviceptr>(args, L.off_in_val + 8 * j, ins[j].val);
-    Put<CUdeviceptr>(args, L.off_in_vld + 8 * j, ins[j].vld);
-    Put<CUdeviceptr>(args, L.off_in_var + 8 * j, ins[j].var);
-    Put<uint32_t>(args, L.off_in_vsh + 4 * j, ins[j].vsh);
-    Put<uint32_t>(args, L.off_in_dsh + 4 * j, ins[j].dsh);
-  }
+  PutInputs(args, L, ins);
   // selection vector
   if (selection_mode_ != GDV_SEL_NONE) {
     CUdeviceptr dsel = reinterpret_cast<CUdeviceptr>(sel->indices);
@@ -1188,8 +1266,91 @@ Status Filter::Make(SchemaPtr schema, ConditionPtr cond, const Config& cfg,
   }
   if (std::getenv("GDV_EAGER_NONULL") != nullptr)
     GDV_RETURN_NOT_OK(f->KernelFor(GDV_SEL_UINT32, false, true, &k));
+  // A condition over one dictionary column that no null can satisfy: evaluate it once per entry
+  // (a Projector over the dictionary) and keep rows by their index (DESIGN.md §3.6).
+  const int dc = DictionaryFirstColumn(*schema, *cond->root());
+  if (dc >= 0) {
+    const Field& fd = schema->fields()[static_cast<size_t>(dc)];
+    auto entries = std::make_shared<Schema>(std::vector<Field>{Field{fd.name, fd.type.value_type()}});
+    NodePtr truth = std::make_shared<FunctionNode>("istrue", NodeVector{WithValueTypes(cond->root())}, boolean());
+    GDV_RETURN_NOT_OK(Projector::Make(entries, {std::make_shared<Expression>(truth, Field{"keep", boolean()})},
+                                      GDV_SEL_NONE, cfg, &f->dict_entries_));
+    f->dict_column_ = dc;
+  }
   *out = std::move(f);
   return Status::OK();
+}
+
+Status Filter::LaunchDictionaryFirst(Device* dev, const gdv_batch_t* batch, CUstream stream, bool async, bool large,
+                                     CUdeviceptr d_bits, CUdeviceptr d_idx, int idx_width, CUdeviceptr d_count,
+                                     CUdeviceptr d_state, int64_t n_tiles, int64_t row_base, int64_t out_cap,
+                                     ScratchScope* scratch) {
+  const bool host = batch->mem_space == GDV_MEM_HOST;
+  const int64_t n = batch->num_rows;
+  const gdv_column_t& c = batch->columns[dict_column_];
+  const auto* dict = static_cast<const gdv_dictionary_t*>(c.var_data);
+  if (dict == nullptr || dict->length < 0 || dict->offset < 0)
+    return Status::Make(GDV_INVALID, "dictionary column " + std::to_string(dict_column_) +
+                                         " has no valid dictionary (var_data must point at a gdv_dictionary_t)");
+  const int64_t dlen = dict->length;
+  const size_t words = static_cast<size_t>((dlen + 31) / 32);
+  // 1. the condition over every entry: the dictionary is a one-column batch of its value type
+  if (dlen > 0) {
+    gdv_column_t dc;
+    dc.validity = dict->validity;
+    dc.values = dict->offsets;
+    dc.var_data = dict->data;
+    dc.offset = dict->offset;
+    dc.var_data_size = dict->data_size;
+    const gdv_batch_t db{dlen, 1, batch->mem_space, &dc};
+    gdv_out_column_t out;
+    std::memset(&out, 0, sizeof(out));
+    std::vector<uint32_t> hbits;
+    if (host) {
+      hbits.assign(words + 2, 0u);
+      out.values = hbits.data();
+    } else {
+      out.values = reinterpret_cast<void*>(d_bits);
+    }
+    GDV_RETURN_NOT_OK(dict_entries_->Evaluate(&db, nullptr, &out, 1, stream, !host && async));
+    if (host) GDV_RETURN_NOT_OK(StagedHtoD(dev, d_bits, hbits.data(), words * 4, stream));
+  }
+  // 2. the rows: indices and their validity only
+  const DataType it(schema_->fields()[static_cast<size_t>(dict_column_)].type.index);
+  const int w = it.width();
+  const uint8_t* p = static_cast<const uint8_t*>(c.values) + c.offset * w;
+  if (c.values == nullptr) return Status::Make(GDV_INVALID, "dictionary column has no indices buffer");
+  CUdeviceptr d_in = 0, d_vld = 0;
+  uint32_t vsh = 0;
+  if (host) {
+    GDV_RETURN_NOT_OK(scratch->Alloc(static_cast<size_t>(n) * w + 16, &d_in));
+    GDV_RETURN_NOT_OK(StagedHtoD(dev, d_in, p, static_cast<size_t>(n) * w, stream));
+  } else {
+    if (reinterpret_cast<uintptr_t>(p) % static_cast<uintptr_t>(w) != 0)
+      return Status::Make(GDV_INVALID, "device indices buffer of column " + std::to_string(dict_column_) +
+                                           " is not aligned to its element width");
+    d_in = reinterpret_cast<CUdeviceptr>(p);
+  }
+  if (c.validity != nullptr)
+    GDV_RETURN_NOT_OK(ResolveBitmap(dev, c.validity, c.offset, n, host, stream, scratch, &d_vld, &vsh));
+  const std::string name = std::string("gdv_dict_filter_") + it.ctype() + (large ? "_w4" : "_w1");
+  CUfunction fn = nullptr;
+  GDV_RETURN_NOT_OK(dev->StaticFunction(name.c_str(), &fn));
+  // the entry bitmap lives in shared memory up to 64 K entries (8 KB per CTA, DESIGN.md §3.6)
+  int smem_words = dlen <= 65536 ? static_cast<int>(words) : 0;
+  const size_t smem = static_cast<size_t>(smem_words) * 4;
+  const DriverApi& d = Driver();
+  int per_sm = 1;
+  if (d.OccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, smem) != CUDA_SUCCESS || per_sm < 1) per_sm = 1;
+  const int64_t cap = static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * per_sm;
+  const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap)));
+  CUdeviceptr tile_state = d_state + 16, ticket = d_state;
+  int64_t nn = n, rb = row_base, oc = out_cap, dl = dlen;
+  int ow = idx_width;
+  void* params[] = {&d_in, &d_vld, &vsh, &d_bits, &dl, &smem_words, &nn, &rb, &d_idx, &ow, &d_count, &tile_state, &ticket, &oc};
+  g_launch_count.fetch_add(1);
+  return CuCheck(d.LaunchKernel(fn, grid, 1, 1, 256, 1, 1, static_cast<unsigned>(smem), stream, params, nullptr),
+                 "cuLaunchKernel(gdv_dict_filter)");
 }
 
 Status Filter::KernelFor(int mode, bool nullable, bool large, CompiledKernel** out) {
@@ -1260,31 +1421,34 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
 
   Device* dev = nullptr;
   GDV_RETURN_NOT_OK(Device::Get(cfg_.device, &dev));
-  CompiledKernel* general = nullptr;
-  GDV_RETURN_NOT_OK(KernelFor(GDV_SEL_UINT32, true, false, &general));
-  CompiledKernel* kernel = nullptr;
   const bool large = batch->num_rows >= (int64_t(32) << 20);
-  GDV_RETURN_NOT_OK(
-      KernelFor(sel_mode, AnyValidity(general->gen, batch), large, &kernel));
-  last_used_ = kernel;
+  const bool dict_first = dict_entries_ != nullptr;
+  dict_first_used_ = dict_first;
+  CompiledKernel* kernel = nullptr;
   CompiledKernel::Loaded l;
-  GDV_RETURN_NOT_OK(kernel->Load(dev, &l));
+  if (!dict_first) {
+    CompiledKernel* general = nullptr;
+    GDV_RETURN_NOT_OK(KernelFor(GDV_SEL_UINT32, true, false, &general));
+    GDV_RETURN_NOT_OK(KernelFor(sel_mode, AnyValidity(general->gen, batch), large, &kernel));
+    last_used_ = kernel;
+    GDV_RETURN_NOT_OK(kernel->Load(dev, &l));
+  }
   const DriverApi& d = Driver();
   CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
-  const GeneratedKernel& gen = kernel->gen;
 
   ScratchScope scratch(dev);
   scratch.Guard(stream);
   std::vector<ResolvedIn> ins;
-  GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
+  if (!dict_first) GDV_RETURN_NOT_OK(ResolveInputs(dev, kernel->gen, batch, stream, &scratch, &ins));
 
-  // Row tiles: ceil(n / tile_rows) look-back descriptors.
-  const int64_t tile_rows = gen.tile_rows;
+  // Row tiles: ceil(n / tile_rows) look-back descriptors (the dictionary-first kernel: 8 warps x W
+  // 1024-row chunks, W = 4 on big batches like the fused filter's).
+  const int64_t tile_rows = dict_first ? int64_t(8 * 1024) * (large ? 4 : 1) : kernel->gen.tile_rows;
   const int64_t n_tiles = (n + tile_rows - 1) / tile_rows;
 
   // Per-stream persistent scratch: [ticket u64][count u64][tile_state n_tiles x u64]
   const size_t state_bytes = 16 + static_cast<size_t>(n_tiles) * 8;
-  CUdeviceptr d_state = 0, d_err = 0;
+  CUdeviceptr d_state = 0, d_err = 0, d_bits = 0;
   {
     std::lock_guard<std::mutex> lock(mu_);
     Pending& pend = pending_[stream];
@@ -1296,7 +1460,18 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
       pend.state_cap = state_bytes;
     }
     d_state = pend.d_state;
-    if (gen.uses_ctx) {
+    if (dict_first) {
+      const auto* dict = static_cast<const gdv_dictionary_t*>(batch->columns[dict_column_].var_data);
+      const int64_t dlen = dict != nullptr ? dict->length : 0;
+      const size_t bits_bytes = static_cast<size_t>(std::max<int64_t>(dlen, 0) + 31) / 32 * 4 + 16;
+      if (pend.bits_cap < bits_bytes) {
+        GDV_RETURN_NOT_OK(dev->Alloc(bits_bytes, &pend.d_bits));
+        pend.scratch.push_back(pend.d_bits);
+        pend.bits_cap = bits_bytes;
+      }
+      d_bits = pend.d_bits;
+    }
+    if (!dict_first && kernel->gen.uses_ctx) {
       if (pend.d_err == 0) {
         GDV_RETURN_NOT_OK(dev->Alloc(256, &pend.d_err));
         GDV_RETURN_NOT_OK(CuCheck(d.MemsetD8Async(pend.d_err, 0, 256, stream), "memset err"));
@@ -1318,27 +1493,27 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
   const int iw = SelWidth(sel_mode);
   if (host) GDV_RETURN_NOT_OK(scratch.Alloc(static_cast<size_t>(n) * iw + 16, &d_idx));
 
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), 0);
-  std::vector<uint8_t> args(L.size, 0);
-  Put<int64_t>(args, L.off_n, n);
-  Put<int64_t>(args, L.off_row_base, out_sel->index_base);
-  Put<CUdeviceptr>(args, L.off_out_idx, d_idx);
-  Put<CUdeviceptr>(args, L.off_out_count, d_count);
-  Put<CUdeviceptr>(args, L.off_tile_state, d_state + 16);
-  Put<CUdeviceptr>(args, L.off_ticket, d_state);
-  Put<CUdeviceptr>(args, L.off_err, d_err);
-  Put<int64_t>(args, L.off_out_cap, bounded ? out_sel->max_slots : n);
-  for (size_t j = 0; j < ins.size(); ++j) {
-    Put<CUdeviceptr>(args, L.off_in_val + 8 * j, ins[j].val);
-    Put<CUdeviceptr>(args, L.off_in_vld + 8 * j, ins[j].vld);
-    Put<CUdeviceptr>(args, L.off_in_var + 8 * j, ins[j].var);
-    Put<uint32_t>(args, L.off_in_vsh + 4 * j, ins[j].vsh);
-    Put<uint32_t>(args, L.off_in_dsh + 4 * j, ins[j].dsh);
+  if (dict_first) {
+    GDV_RETURN_NOT_OK(LaunchDictionaryFirst(dev, batch, stream, async, large, d_bits, d_idx, iw, d_count, d_state, n_tiles,
+                                            out_sel->index_base, bounded ? out_sel->max_slots : n, &scratch));
+  } else {
+    const GeneratedKernel& gen = kernel->gen;
+    ArgsLayout L(static_cast<int>(gen.inputs.size()), 0, HasDictionary(gen.inputs));
+    std::vector<uint8_t> args(L.size, 0);
+    Put<int64_t>(args, L.off_n, n);
+    Put<int64_t>(args, L.off_row_base, out_sel->index_base);
+    Put<CUdeviceptr>(args, L.off_out_idx, d_idx);
+    Put<CUdeviceptr>(args, L.off_out_count, d_count);
+    Put<CUdeviceptr>(args, L.off_tile_state, d_state + 16);
+    Put<CUdeviceptr>(args, L.off_ticket, d_state);
+    Put<CUdeviceptr>(args, L.off_err, d_err);
+    Put<int64_t>(args, L.off_out_cap, bounded ? out_sel->max_slots : n);
+    PutInputs(args, L, ins);
+    const int64_t cap =
+        static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * l.blocks_per_sm;
+    const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap)));
+    GDV_RETURN_NOT_OK(LaunchKernel(dev, l, gen, args, grid, stream));
   }
-  const int64_t cap =
-      static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * l.blocks_per_sm;
-  const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap)));
-  GDV_RETURN_NOT_OK(LaunchKernel(dev, l, gen, args, grid, stream));
 
   out_sel->num_slots = -1;
   if (host) {

@@ -163,6 +163,8 @@ struct Pending {
   CUdeviceptr d_count = 0;
   CUdeviceptr d_state = 0;  // filter look-back state, reused by stream-ordered launches
   size_t state_cap = 0;
+  CUdeviceptr d_bits = 0;   // dictionary-first filter: one bit per dictionary entry
+  size_t bits_cap = 0;
   bool uses_ctx = false;
 };
 
@@ -234,8 +236,20 @@ class Filter {
   const Config& config() const { return cfg_; }
   const SchemaPtr& schema() const { return schema_; }
   CompiledKernel* last_used() const { return rope_main_ != nullptr ? rope_main_->last_used() : last_used_.load(); }
+  // 1 when the latest Evaluate took the dictionary-first path (DESIGN.md §3.6).
+  bool dictionary_first_used() const { return dict_first_used_.load(); }
 
  private:
+  // Dictionary-first plan (DictionaryFirstColumn): `dict_entries_` evaluates istrue(condition) over the
+  // dictionary of column `dict_column_` seen as a one-column batch, one bit per entry; the rows are then
+  // kept by the static gdv_dict_filter_* kernel from their indices alone.
+  std::shared_ptr<Projector> dict_entries_;
+  int dict_column_ = -1;
+  std::atomic<bool> dict_first_used_{false};
+  Status LaunchDictionaryFirst(Device* dev, const gdv_batch_t* batch, CUstream stream, bool async, bool large,
+                               CUdeviceptr d_bits, CUdeviceptr d_idx, int idx_width, CUdeviceptr d_count,
+                               CUdeviceptr d_state, int64_t n_tiles, int64_t row_base, int64_t out_cap,
+                               ScratchScope* scratch);
   std::shared_ptr<Projector> rope_pre_;  // consumers of a rope (gdv_rope_temps.h): temps first,
   std::shared_ptr<Filter> rope_main_;    // then the condition over the batch plus the temp columns
   std::atomic<CompiledKernel*> last_used_{nullptr};

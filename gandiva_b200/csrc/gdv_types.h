@@ -8,15 +8,36 @@
 
 namespace gdv {
 
+// A dictionary-encoded column (arrow::DictionaryType) is its value type plus the index type:
+// `id` is the value type's id, `index` the signed integer id of the indices (0 = plain column).
+// Everything that reads values -- function resolution, if/else and IN type checks -- sees the
+// value type; operator== compares value types, same() also the encoding.  At the C-ABI it is
+// GDV_TYPE_DICTIONARY (include/gandiva_b200.h).
 struct DataType {
   int32_t id = GDV_TYPE_NA;
   int32_t precision = 0;  // decimal precision, or time unit for timestamp/time
   int32_t scale = 0;
+  int32_t index = 0;      // dictionary columns: GDV_TYPE_INT8..INT64 (or what the caller sent)
+  bool ordered = false;   // dictionary columns: DictionaryType::ordered
 
   DataType() = default;
   DataType(int32_t i, int32_t p = 0, int32_t s = 0) : id(i), precision(p), scale(s) {}
-  explicit DataType(const gdv_type_t& t) : id(t.id), precision(t.precision), scale(t.scale) {}
-  gdv_type_t c() const { return gdv_type_t{id, precision, scale}; }
+  explicit DataType(const gdv_type_t& t) : id(t.id), precision(t.precision), scale(t.scale) {
+    if (t.id == GDV_TYPE_DICTIONARY) {
+      id = t.scale;
+      index = t.precision & 0xff;
+      ordered = (t.precision & GDV_DICT_ORDERED) != 0;
+      precision = scale = 0;
+    }
+  }
+  gdv_type_t c() const {
+    if (index != 0) return gdv_type_t{GDV_TYPE_DICTIONARY, index | (ordered ? GDV_DICT_ORDERED : 0), id};
+    return gdv_type_t{id, precision, scale};
+  }
+  bool is_dict() const { return index != 0; }
+  // The type of the values (the dictionary's type for a dictionary column).
+  DataType value_type() const { return DataType(id, precision, scale); }
+  bool same(const DataType& o) const { return *this == o && index == o.index && ordered == o.ordered; }
 
   bool operator==(const DataType& o) const {
     if (id != o.id) return false;

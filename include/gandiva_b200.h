@@ -83,11 +83,19 @@ typedef int32_t gdv_status;
 #define GDV_TYPE_TIME32 19
 #define GDV_TYPE_TIME64 20
 #define GDV_TYPE_DECIMAL128 23
+/* Dictionary-encoded column (arrow::DictionaryType): precision = index type id (GDV_TYPE_INT8,
+ * INT16, INT32 or INT64), OR'ed with GDV_DICT_ORDERED for an ordered dictionary; scale = value
+ * type id (GDV_TYPE_STRING or GDV_TYPE_BINARY).  Input columns only: functions resolve against
+ * the value type, and results are plain utf8 / binary.  Any other value or index type, and a
+ * dictionary result type, is refused at Make() with GDV_NOT_IMPLEMENTED. */
+#define GDV_TYPE_DICTIONARY 29
+#define GDV_DICT_ORDERED 0x100
 
 typedef struct gdv_type {
   int32_t id;        /* GDV_TYPE_* */
-  int32_t precision; /* decimal128: precision; timestamp/time: arrow::TimeUnit (0=s,1=ms,2=us,3=ns) */
-  int32_t scale;     /* decimal128: scale */
+  int32_t precision; /* decimal128: precision; timestamp/time: arrow::TimeUnit (0=s,1=ms,2=us,3=ns);
+                        dictionary: index type id (| GDV_DICT_ORDERED) */
+  int32_t scale;     /* decimal128: scale; dictionary: value type id */
 } gdv_type_t;
 
 /* ---- opaque handles ----------------------------------------------------- */
@@ -149,6 +157,25 @@ typedef struct gdv_column {
   int64_t offset;
   int64_t var_data_size; /* bytes in var_data (needed to stage host strings); 0 otherwise */
 } gdv_column_t;
+
+/* The dictionary of a dictionary-encoded column (schema type GDV_TYPE_DICTIONARY): a utf8 /
+ * binary array in the batch's memory space, described like a gdv_column_t plus its length.
+ * The column itself is
+ *  dictionary  : validity | signed int8/16/32/64 indices (values) | var_data = const gdv_dictionary_t*
+ * with `offset` applying to the indices and this struct's `offset` to the dictionary, so the
+ * layout of gdv_column_t / gdv_batch_t is the same for every column kind.  Row r is
+ * dictionary[indices[r]]; it is null when the index slot or the dictionary entry is null, and
+ * also when the index lies outside [0, length) (invalid Arrow input: never dereferenced).  Host
+ * batches stage the three dictionary buffers with the indices; device batches read them in place.
+ * The struct is read during the Evaluate call only (host memory). */
+typedef struct gdv_dictionary {
+  const void* validity;  /* may be NULL (no null entries) */
+  const void* offsets;   /* length + 1 int32 offsets, from `offset` on */
+  const void* data;      /* the bytes the offsets index */
+  int64_t offset;        /* ArrayData::offset of the dictionary */
+  int64_t length;        /* entries */
+  int64_t data_size;     /* bytes in data (needed to stage host dictionaries) */
+} gdv_dictionary_t;
 
 typedef struct gdv_batch {
   int64_t num_rows;
@@ -273,6 +300,8 @@ int64_t gdv_filter_dump_ir(gdv_filter_t f, char* buf, int64_t buf_len);
 gdv_status gdv_filter_kernel_info(gdv_filter_t f, char* name_buf, int64_t name_len, int32_t* regs,
                                   int32_t* smem_bytes, int32_t* rows_per_thread,
                                   int32_t* block_threads);
+/* Same keys as gdv_projector_kernel_attr, plus "dictionary_first": 1 when the latest Evaluate kept rows
+ * through the dictionary-first kernel (a condition over one dictionary column, evaluated once per entry). */
 gdv_status gdv_filter_kernel_attr(gdv_filter_t f, const char* key, int64_t* out);
 void gdv_filter_release(gdv_filter_t f);
 
