@@ -81,6 +81,14 @@ class gdv_dictionary_t(C.Structure):
                 ("offset", C.c_int64), ("length", C.c_int64), ("data_size", C.c_int64)]
 
 
+class gdv_view_buffers_t(C.Structure):
+    """The data buffers of a string_view / binary_view column (include/gandiva_b200.h): the column's
+    gdv_column_t holds validity + 16-byte views, and its var_data points at one of these.  `data` is
+    a host array of `n` buffer pointers and `sizes` their n int64 sizes, both in the batch's memory
+    space (device pointers and a device sizes array for evaluate_device)."""
+    _fields_ = [("data", C.POINTER(C.c_void_p)), ("sizes", C.c_void_p), ("n", C.c_int32)]
+
+
 class gdv_batch_t(C.Structure):
     _fields_ = [("num_rows", C.c_int64), ("num_columns", C.c_int32), ("mem_space", C.c_int32),
                 ("columns", C.POINTER(gdv_column_t))]
@@ -218,6 +226,8 @@ _UNIT = {"s": 0, "ms": 1, "us": 2, "ns": 3}
 
 GDV_TYPE_DICTIONARY = 29
 GDV_DICT_ORDERED = 0x100
+GDV_TYPE_STRING_VIEW = 39
+GDV_TYPE_BINARY_VIEW = 40
 
 
 def _to_c_type(t: pa.DataType) -> gdv_type_t:
@@ -236,7 +246,7 @@ def _from_c_type(t: gdv_type_t) -> pa.DataType:
     simple = {1: pa.bool_(), 2: pa.uint8(), 3: pa.int8(), 4: pa.uint16(), 5: pa.int16(),
               6: pa.uint32(), 7: pa.int32(), 8: pa.uint64(), 9: pa.int64(), 11: pa.float32(),
               12: pa.float64(), 13: pa.string(), 14: pa.binary(), 16: pa.date32(),
-              17: pa.date64()}
+              17: pa.date64(), GDV_TYPE_STRING_VIEW: pa.string_view(), GDV_TYPE_BINARY_VIEW: pa.binary_view()}
     if tid in simple:
         return simple[tid]
     if tid == GDV_TYPE_DICTIONARY:
@@ -580,6 +590,29 @@ def _dictionary_to_c(d: pa.Array) -> gdv_dictionary_t:
     return c
 
 
+def view_buffers(data: Sequence[int], sizes: int) -> gdv_view_buffers_t:
+    """gdv_view_buffers_t over `data` (buffer addresses) and `sizes` (address of len(data) int64
+    sizes), e.g. device pointers for Projector / Filter evaluate_device."""
+    c = gdv_view_buffers_t()
+    table = (C.c_void_p * max(len(data), 1))(*[int(p) or None for p in data])
+    c.data = C.cast(table, C.POINTER(C.c_void_p))
+    c.sizes = sizes or None
+    c.n = len(data)
+    c._keep = table
+    return c
+
+
+def _view_buffers_to_c(arr: pa.Array) -> gdv_view_buffers_t:
+    """The data buffers of a string_view / binary_view array (sliced ones included: a slice keeps
+    every buffer of its parent) -> gdv_view_buffers_t with host pointers.  pyarrow lists them as
+    buffers()[2:], without the variadic sizes buffer: the sizes are the buffers' own sizes."""
+    data = [b for b in arr.buffers()[2:]]
+    sizes = np.array([b.size if b is not None else 0 for b in data] or [0], dtype=np.int64)
+    c = view_buffers([b.address if b is not None else 0 for b in data], sizes.ctypes.data)
+    c._keep = (c._keep, data, sizes)
+    return c
+
+
 def _batch_to_c(batch: pa.RecordBatch):
     """RecordBatch -> gdv_batch_t over the batch's own buffers (no copies)."""
     cols = (gdv_column_t * max(batch.num_columns, 1))()
@@ -598,6 +631,12 @@ def _batch_to_c(batch: pa.RecordBatch):
             d = _dictionary_to_c(arr.dictionary)
             keep.append(d)
             c.var_data = C.addressof(d)
+        elif pa.types.is_string_view(t) or pa.types.is_binary_view(t):
+            # views like a fixed-width column; var_data -> the data buffers (zero copy)
+            c.values = bufs[1].address if bufs[1] is not None else None
+            v = _view_buffers_to_c(arr)
+            keep.append(v)
+            c.var_data = C.addressof(v)
         elif pa.types.is_string(t) or pa.types.is_binary(t):
             c.values = bufs[1].address if bufs[1] is not None else None
             c.var_data = bufs[2].address if len(bufs) > 2 and bufs[2] is not None else None
@@ -610,9 +649,9 @@ def _batch_to_c(batch: pa.RecordBatch):
 
 
 def _var_ptr(var):
-    """var_data of a device column: the bytes of a utf8 / binary column, or a gdv_dictionary_t (with
-    device pointers) for a dictionary-encoded one."""
-    if isinstance(var, gdv_dictionary_t):
+    """var_data of a device column: the bytes of a utf8 / binary column, a gdv_dictionary_t (with
+    device pointers) for a dictionary-encoded one, or a gdv_view_buffers_t for a view column."""
+    if isinstance(var, (gdv_dictionary_t, gdv_view_buffers_t)):
         return C.addressof(var)
     return var or None
 
@@ -649,6 +688,7 @@ def _kernel_info(fn, handle, attr_fn=None) -> dict:
             "rows_per_thread": rpt.value, "block_threads": bt.value}
     if attr_fn is not None:
         keys = ["staged", "stages", "dynamic_smem", "cta_tile_rows", "tile_rows", "nullable"]
+        keys.append("view_shortcuts")
         if attr_fn is lib.gdv_filter_kernel_attr:
             keys.append("dictionary_first")
         if regs.value >= 0:
@@ -732,7 +772,8 @@ class Projector:
     def evaluate_device(self, num_rows: int, columns: Sequence[tuple], outputs: Sequence[tuple],
                         stream: int = 0, selection: tuple | None = None, sync: bool = False) -> None:
         """columns: per schema field (validity_ptr|0, values_ptr, var_data_ptr|0, offset), where a
-        dictionary-encoded column passes its indices as values and a gdv_dictionary_t as var_data;
+        dictionary-encoded column passes its indices as values and a gdv_dictionary_t as var_data, and
+        a string_view / binary_view column its 16-byte views and a gdv_view_buffers_t (view_buffers());
         outputs: per expression (validity_ptr|0, values_ptr); selection: (ptr, num_slots) or
         (ptr, max_slots, d_count_ptr): the slot count is read from device memory (the d_count a
         Filter.evaluate_device(..., sync=False) wrote on the same stream), no host round trip."""

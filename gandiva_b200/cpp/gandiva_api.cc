@@ -2,6 +2,7 @@
 // implemented as a thin layer over the C-ABI of libgandiva_b200.so.  Links libarrow only for
 // the Arrow types that appear in the signatures (RecordBatch, Array, MemoryPool, Status).
 #include <cstring>
+#include <memory>
 
 #include "arrow/array/util.h"
 #include "arrow/buffer.h"
@@ -62,6 +63,8 @@ DataTypePtr FromC(const gdv_type_t& t) {
     case GDV_TYPE_DOUBLE: return arrow::float64();
     case GDV_TYPE_STRING: return arrow::utf8();
     case GDV_TYPE_BINARY: return arrow::binary();
+    case GDV_TYPE_STRING_VIEW: return arrow::utf8_view();
+    case GDV_TYPE_BINARY_VIEW: return arrow::binary_view();
     case GDV_TYPE_DATE32: return arrow::date32();
     case GDV_TYPE_DATE64: return arrow::date64();
     case GDV_TYPE_TIMESTAMP: return arrow::timestamp(static_cast<arrow::TimeUnit::type>(t.precision));
@@ -174,12 +177,23 @@ gdv_config_t ConfigToC(const std::shared_ptr<Configuration>& c) {
   return cfg;
 }
 
+// The data buffers of a string_view / binary_view column (buffers[2..] of its ArrayData), held for
+// one Evaluate call: the pointer table, the sizes (copied into device memory for a device batch) and
+// the gdv_view_buffers_t the column's var_data points at.
+struct ViewBuffers {
+  std::vector<const void*> data;
+  std::vector<int64_t> sizes;
+  std::shared_ptr<arrow::Buffer> device_sizes;
+  std::shared_ptr<arrow::MemoryManager> mm;
+  gdv_view_buffers_t c{};
+};
+
 // RecordBatch -> raw buffer addresses (arrow::ArrayData, P/include/arrow/array/data.h:468-474).
 // All buffers of a batch must live in one memory space: CPU (GDV_MEM_HOST, staged by the engine) or the
 // HBM of one GPU (GDV_MEM_DEVICE: kernels read them in place).  *mm = the MemoryManager of the first
-// device buffer, from which device outputs are allocated.
+// device buffer, from which device outputs are allocated.  View columns' descriptors go to *views.
 Status ToColumns(const arrow::RecordBatch& batch, std::vector<gdv_column_t>* cols, int* mem_space,
-                 std::shared_ptr<arrow::MemoryManager>* mm) {
+                 std::shared_ptr<arrow::MemoryManager>* mm, std::vector<std::unique_ptr<ViewBuffers>>* views) {
   int n_cpu = 0, n_dev = 0;
   for (int i = 0; i < batch.num_columns(); ++i) {
     const arrow::ArrayData& a = *batch.column_data(i);
@@ -203,7 +217,21 @@ Status ToColumns(const arrow::RecordBatch& batch, std::vector<gdv_column_t>* col
     if (a.buffers.size() > 0 && a.buffers[0] != nullptr && a.null_count.load() != 0)
       c.validity = reinterpret_cast<const void*>(a.buffers[0]->address());
     if (a.buffers.size() > 1 && a.buffers[1] != nullptr) c.values = reinterpret_cast<const void*>(a.buffers[1]->address());
-    if (a.buffers.size() > 2 && a.buffers[2] != nullptr) {
+    const auto tid = a.type->id();
+    if (tid == arrow::Type::STRING_VIEW || tid == arrow::Type::BINARY_VIEW) {
+      auto v = std::make_unique<ViewBuffers>();
+      for (size_t k = 2; k < a.buffers.size(); ++k) {
+        const auto& b = a.buffers[k];
+        v->data.push_back(b != nullptr ? reinterpret_cast<const void*>(b->address()) : nullptr);
+        v->sizes.push_back(b != nullptr ? b->size() : 0);
+        if (b != nullptr && !b->is_cpu() && v->mm == nullptr) v->mm = b->memory_manager();
+      }
+      v->c.data = v->data.data();
+      v->c.sizes = v->sizes.data();
+      v->c.n = static_cast<int32_t>(v->data.size());
+      c.var_data = &v->c;
+      views->push_back(std::move(v));
+    } else if (a.buffers.size() > 2 && a.buffers[2] != nullptr) {
       c.var_data = reinterpret_cast<const void*>(a.buffers[2]->address());
       c.var_data_size = a.buffers[2]->size();
     }
@@ -213,6 +241,17 @@ Status ToColumns(const arrow::RecordBatch& batch, std::vector<gdv_column_t>* col
   if (n_cpu > 0 && n_dev > 0)
     return Status::Invalid("the buffers of a RecordBatch must all be in host memory or all in device memory");
   *mem_space = n_dev > 0 ? GDV_MEM_DEVICE : GDV_MEM_HOST;
+  if (*mem_space == GDV_MEM_DEVICE) {
+    // the engine reads a device batch's view sizes on the device
+    for (auto& v : *views) {
+      if (v->sizes.empty()) continue;
+      if (v->mm == nullptr) return Status::Invalid("a device string_view column has no device data buffer");
+      auto host = std::make_shared<arrow::Buffer>(reinterpret_cast<const uint8_t*>(v->sizes.data()),
+                                                  static_cast<int64_t>(v->sizes.size() * 8));
+      ARROW_ASSIGN_OR_RAISE(v->device_sizes, arrow::MemoryManager::CopyBuffer(host, v->mm));
+      v->c.sizes = reinterpret_cast<const int64_t*>(v->device_sizes->address());
+    }
+  }
   return Status::OK();
 }
 
@@ -541,7 +580,8 @@ Status Projector::Evaluate(const arrow::RecordBatch& batch, const SelectionVecto
   std::vector<gdv_column_t> cols;
   int space = GDV_MEM_HOST;
   std::shared_ptr<arrow::MemoryManager> mm;
-  ARROW_RETURN_NOT_OK(ToColumns(batch, &cols, &space, &mm));
+  std::vector<std::unique_ptr<ViewBuffers>> views;
+  ARROW_RETURN_NOT_OK(ToColumns(batch, &cols, &space, &mm, &views));
   const bool on_device = space == GDV_MEM_DEVICE;
   gdv_batch_t b{batch.num_rows(), batch.num_columns(), space, cols.data()};
   const int64_t n = selection_vector != nullptr && mode_ != SelectionVector::MODE_NONE
@@ -646,7 +686,8 @@ Status Filter::Evaluate(const arrow::RecordBatch& batch, std::shared_ptr<Selecti
     return Status::Invalid("Output selection vector capacity too small");
   std::vector<gdv_column_t> cols;
   int space = GDV_MEM_HOST;
-  ARROW_RETURN_NOT_OK(ToColumns(batch, &cols, &space, nullptr));
+  std::vector<std::unique_ptr<ViewBuffers>> views;
+  ARROW_RETURN_NOT_OK(ToColumns(batch, &cols, &space, nullptr, &views));
   if (out_selection->GetBuffer().is_cpu() == (space == GDV_MEM_DEVICE))
     return Status::Invalid("the selection vector and the RecordBatch must live in the same memory space "
                            "(SelectionVector::MakeInt32(max_slots, <device buffer>, &out) for device batches)");

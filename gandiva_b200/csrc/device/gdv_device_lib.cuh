@@ -226,6 +226,63 @@ GDV_DEV gdv_str gdv_dict_view(const i32* dof, const u8* dat, const u32* dvl, u32
   *ok = v;
   return gdv_make_str(dat + a, b - a);
 }
+// One 16-byte view of a string_view / binary_view column.  Read through the ordinary cached path,
+// not ld.global.cs like the fixed-width columns: the inline bytes of a short string are read back
+// through the row's gdv_str (which points into the view in global memory), and an evict-first line
+// may be gone by then.
+GDV_DEV uint4 gdv_ldview(const uint4* p) { return __ldg(p); }
+// Row view of a string_view / binary_view column: `v` is the row's view as loaded from `at`
+// ({len, prefix or bytes 0..3, buffer index or bytes 4..7, offset or bytes 8..11}), `bufs` / `sizes` /
+// `nb` the column's data buffers.  A string of <= 12 bytes points at bytes 4.. of the view itself
+// (global memory, so the string write pass's warp-cooperative copy reads it like any other bytes);
+// a longer one at bufs[index] + offset.  *ok = the view is valid: a negative length, a buffer index
+// outside [0, nb), a negative offset or offset + len past the buffer's size is invalid Arrow input.
+// Its row reads as null and nothing is dereferenced for it (the view is empty).
+GDV_DEV gdv_str gdv_sv_view(const uint4& v, const uint4* at, const u8* const* bufs, const i64* sizes, i64 nb,
+                            bool* ok) {
+  const i32 len = (i32)v.x;
+  const u8* inl = reinterpret_cast<const u8*>(at) + 4;
+  if (len <= 12) {
+    *ok = len >= 0;
+    return gdv_make_str(inl, len >= 0 ? len : 0);
+  }
+  const i32 bi = (i32)v.z, off = (i32)v.w;
+  bool good = bi >= 0 && (i64)bi < nb && off >= 0;
+  if (good) good = (i64)off + (i64)len <= __ldg(sizes + bi);
+  *ok = good;
+  if (!good) return gdv_make_str(inl, 0);
+  const u8* base = reinterpret_cast<const u8*>(__ldg(reinterpret_cast<const unsigned long long*>(bufs) + bi));
+  return gdv_make_str(base + off, len);
+}
+// Mask of the first k bytes (k clamped to [0, 4]) of a little-endian word.
+GDV_DEV u32 gdv_bytemask(i32 k) { return k <= 0 ? 0u : k >= 4 ? 0xffffffffu : (1u << (8 * k)) - 1u; }
+// Bytes [4, n) of a string against bytes [4, n) of a literal (the first four agreed already).
+GDV_DEV bool gdv_sv_tail_eq(const u8* p, const u8* lit, i32 n) {
+  for (i32 i = 4; i < n; ++i)
+    if (p[i] != lit[i]) return false;
+  return true;
+}
+// Inline / prefix shortcut (DESIGN.md §3.7).  The literal's first 12 bytes arrive as words a, b, c
+// (zero padded), its length n / m as a constant, so the masks fold.  Bytes after a short string's
+// end are not trusted to be zero: every compare is masked by the length.
+// The row equals the literal: the lengths agree, then the inline words (n <= 12) or the prefix word
+// and the out-of-line bytes through s (n > 12; s.len == n also rules out an invalid view).
+GDV_DEV bool gdv_sv_equal(const uint4& v, const gdv_str& s, i32 n, u32 a, u32 b, u32 c, const u8* lit) {
+  if ((i32)v.x != n) return false;
+  if (n <= 12)
+    return ((v.y ^ a) & gdv_bytemask(n)) == 0u && ((v.z ^ b) & gdv_bytemask(n - 4)) == 0u &&
+           ((v.w ^ c) & gdv_bytemask(n - 8)) == 0u;
+  return v.y == a && s.len == n && gdv_sv_tail_eq(s.p, lit, n);
+}
+// The row starts with the literal (m >= 1): the first min(m, 4) bytes are the same word of an inline
+// and of an out-of-line view.
+GDV_DEV bool gdv_sv_starts(const uint4& v, const gdv_str& s, i32 m, u32 a, u32 b, u32 c, const u8* lit) {
+  const i32 len = (i32)v.x;
+  if (len < m || ((v.y ^ a) & gdv_bytemask(m)) != 0u) return false;
+  if (m <= 4) return true;
+  if (len <= 12) return ((v.z ^ b) & gdv_bytemask(m - 4)) == 0u && ((v.w ^ c) & gdv_bytemask(m - 8)) == 0u;
+  return s.len >= m && gdv_sv_tail_eq(s.p, lit, m);
+}
 // The 32 bitmap bits of rows [rb, rb + 32), rb % 32 == 0, of a bitmap whose row 0 is bit `sh` of the
 // 4-byte aligned word *p; rows >= n read as 0 and no byte past the one that holds row n - 1 is touched.
 // (Filter epilogue: one word per lane and 1024-row chunk, ColumnSlot::hoist.)

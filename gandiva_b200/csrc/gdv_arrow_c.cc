@@ -44,6 +44,8 @@ Status ParseFormat(const char* f, DataType* out) {
   if (s == "g") { *out = DataType(GDV_TYPE_DOUBLE); return Status::OK(); }
   if (s == "u") { *out = DataType(GDV_TYPE_STRING); return Status::OK(); }
   if (s == "z") { *out = DataType(GDV_TYPE_BINARY); return Status::OK(); }
+  if (s == "vu") { *out = DataType(gdv_type_t{GDV_TYPE_STRING_VIEW, 0, 0}); return Status::OK(); }
+  if (s == "vz") { *out = DataType(gdv_type_t{GDV_TYPE_BINARY_VIEW, 0, 0}); return Status::OK(); }
   if (s == "tdD") { *out = DataType(GDV_TYPE_DATE32); return Status::OK(); }
   if (s == "tdm") { *out = DataType(GDV_TYPE_DATE64); return Status::OK(); }
   int u = 0;
@@ -68,6 +70,7 @@ Status ParseFormat(const char* f, DataType* out) {
 
 std::string FormatOf(const DataType& t) {
   static const char kUnit[] = {'s', 'm', 'u', 'n'};
+  if (t.is_view()) return t.id == GDV_TYPE_BINARY ? "vz" : "vu";
   switch (t.id) {
     case GDV_TYPE_BOOL: return "b";
     case GDV_TYPE_INT8: return "c";
@@ -117,6 +120,7 @@ struct gdv_arrow_batch_s {
   SchemaPtr schema;
   std::vector<gdv_column_t> columns;
   std::vector<gdv_dictionary_t> dictionaries;  // dictionary columns' var_data points here
+  std::vector<gdv_view_buffers_t> view_buffers;  // view columns' var_data points here
   gdv_batch_t view;
   int device = -1;  // CUDA ordinal, -1 for host memory
 };
@@ -189,6 +193,9 @@ gdv_status gdv_schema_from_arrow(const struct ArrowSchema* schema, gdv_schema_t*
       // dictionary-encoded: the child's format is the index type's, the dictionary's the values'
       DataType v;
       s = ParseFormat(c->dictionary->format, &v);
+      if (s.ok() && v.is_view())
+        s = Status::Make(GDV_NOT_IMPLEMENTED, "column '" + std::string(c->name ? c->name : "") + "': dictionaries whose "
+                                                  "values are " + v.ToString() + " are not supported");
       if (s.ok() && (!v.is_varlen() || !t.is_signed_integer()))
         s = Status::Make(GDV_NOT_IMPLEMENTED, "column '" + std::string(c->name ? c->name : "") +
                                                   "': dictionaries need utf8 or binary values and signed int8 / int16 / "
@@ -228,16 +235,20 @@ gdv_status gdv_arrow_batch_import(struct ArrowDeviceArray* array, gdv_schema_t s
   b->schema = sch;
   b->device = mem == GDV_MEM_DEVICE ? static_cast<int>(array->device_id) : -1;
   b->dictionaries.assign(fields.size(), gdv_dictionary_t{});
+  b->view_buffers.assign(fields.size(), gdv_view_buffers_t{});
   for (size_t i = 0; i < fields.size(); ++i) {
     const ArrowArray* c = a.children[i];
     const DataType& t = fields[i].type;
     if (c == nullptr) return Fail(GDV_INVALID, "null child array");
+    if (t.is_view() && (c->n_buffers < 3 || c->n_children != 0 || c->dictionary != nullptr))
+      return Fail(GDV_INVALID, "column '" + fields[i].name + "': malformed " + t.ToString() + " array (expected "
+                               "validity, views, the data buffers and their sizes, and no children or dictionary)");
     if (c->n_children != 0) return Fail(GDV_NOT_IMPLEMENTED, "nested columns are not supported");
     if ((c->dictionary != nullptr) != t.is_dict())
       return Fail(c->dictionary != nullptr ? GDV_NOT_IMPLEMENTED : GDV_INVALID,
                   "column '" + fields[i].name + "': the array " + (c->dictionary != nullptr ? "is" : "is not") +
                       " dictionary-encoded but the schema's type is " + t.ToString());
-    const int64_t want = t.is_varlen() && !t.is_dict() ? 3 : 2;
+    const int64_t want = t.is_view() ? c->n_buffers : t.is_varlen() && !t.is_dict() ? 3 : 2;
     if (c->n_buffers != want)
       return Fail(GDV_INVALID, "column '" + fields[i].name + "': expected " + std::to_string(want) +
                                    " buffers, got " + std::to_string(c->n_buffers));
@@ -264,6 +275,14 @@ gdv_status gdv_arrow_batch_import(struct ArrowDeviceArray* array, gdv_schema_t s
       if (mem == GDV_MEM_HOST && d->length > 0)
         dict.data_size = static_cast<const int32_t*>(d->buffers[1])[d->offset + d->length];
       col.var_data = &dict;
+    } else if (t.is_view()) {
+      // zero copy: the producer's buffer array already is the table of data buffers, and its last
+      // buffer the int64 sizes (device memory for a CUDA array: read there by the kernel)
+      gdv_view_buffers_t& vb = b->view_buffers[i];
+      vb.n = static_cast<int32_t>(c->n_buffers - 3);
+      vb.data = c->buffers + 2;
+      vb.sizes = static_cast<const int64_t*>(c->buffers[c->n_buffers - 1]);
+      col.var_data = &vb;
     } else if (t.is_varlen()) {
       col.var_data = c->buffers[2];
       if (mem == GDV_MEM_HOST && c->buffers[1] != nullptr)

@@ -319,6 +319,7 @@ static gdv_status KernelAttr(CompiledKernel& k, const Config& cfg, const char* k
   if (kk == "tile_rows") { *out = k.gen.tile_rows; return GDV_OK; }
   if (kk == "nullable") { *out = k.gen.nullable ? 1 : 0; return GDV_OK; }
   if (kk == "in_bytes_per_row") { *out = k.gen.in_bytes_per_row; return GDV_OK; }
+  if (kk == "view_shortcuts") { *out = k.gen.view_shortcuts; return GDV_OK; }
   if (kk == "blocks_per_sm") {
     Device* dev = nullptr;
     Status s = Device::Get(cfg.device, &dev);

@@ -25,6 +25,12 @@ Status DictionaryResult(const std::string& what) {
                                            "outputs are not supported (results are plain utf8 / binary)");
 }
 
+// string_view / binary_view columns are inputs only, like dictionary-encoded ones.
+Status ViewResult(const std::string& what, const DataType& t) {
+  return Status::Make(GDV_NOT_IMPLEMENTED, "'" + what + "' has a " + t.ToString() + " result type: " + t.ToString() +
+                                           " outputs are not supported (results are plain utf8 / binary)");
+}
+
 bool IsSupportedType(const DataType& t) {
   switch (t.id) {
     case GDV_TYPE_BOOL: case GDV_TYPE_UINT8: case GDV_TYPE_INT8: case GDV_TYPE_UINT16:
@@ -79,7 +85,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
       return Status::OK();
     }
     case NodeKind::kLiteral: {
-      if (!IsSupportedType(node.return_type()) || node.return_type().is_dict())
+      if (!IsSupportedType(node.return_type()) || node.return_type().is_dict() || node.return_type().is_view())
         return VErr("Value " + node.ToString() + " has unsupported data type " +
                     node.return_type().ToString());
       return Status::OK();
@@ -87,6 +93,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
     case NodeKind::kFunction: {
       const auto& fn = static_cast<const FunctionNode&>(node);
       if (fn.return_type().is_dict()) return DictionaryResult(fn.name());
+      if (fn.return_type().is_view()) return ViewResult(fn.name(), fn.return_type());
       std::vector<DataType> params;
       for (const auto& c : fn.children()) {
         Status s = ValidateNode(schema, *c);
@@ -167,6 +174,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
     case NodeKind::kIf: {
       const auto& n = static_cast<const IfNode&>(node);
       if (n.return_type().is_dict()) return DictionaryResult("if");
+      if (n.return_type().is_view()) return ViewResult("if", n.return_type());
       for (const NodePtr* c : {&n.condition(), &n.then_node(), &n.else_node()}) {
         Status s = ValidateNode(schema, **c);
         if (!s.ok()) return s;
@@ -221,6 +229,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
 Status ValidateExpression(const Schema& schema, const Expression& expr) {
   if (expr.root() == nullptr) return VErr("Expression has no root node");
   if (expr.result().type.is_dict()) return DictionaryResult(expr.result().name);
+  if (expr.result().type.is_view()) return ViewResult(expr.result().name, expr.result().type);
   Status s = ValidateNode(schema, *expr.root());
   if (!s.ok()) return s;
   if (expr.root()->return_type() != expr.result().type)
@@ -232,8 +241,8 @@ Status ValidateExpression(const Schema& schema, const Expression& expr) {
 // ======================================================================================
 // Args layout
 // ======================================================================================
-ArgsLayout::ArgsLayout(int n_inputs, int n_outputs, bool dictionary)
-    : ni(std::max(n_inputs, 1)), no(std::max(n_outputs, 1)), dict(dictionary) {
+ArgsLayout::ArgsLayout(int n_inputs, int n_outputs, bool dictionary, bool views)
+    : ni(std::max(n_inputs, 1)), no(std::max(n_outputs, 1)), dict(dictionary), view(views) {
   size_t o = 80;
   off_in_val = o; o += 8u * ni;
   off_in_vld = o; o += 8u * ni;
@@ -250,12 +259,24 @@ ArgsLayout::ArgsLayout(int n_inputs, int n_outputs, bool dictionary)
     off_in_dln = o; o += 8u * ni;
     off_in_dvs = o; o += 4u * ni;
   }
+  if (view) {
+    o = (o + 7u) & ~size_t(7);
+    off_in_vbf = o; o += 8u * ni;
+    off_in_vsz = o; o += 8u * ni;
+    off_in_vbn = o; o += 8u * ni;
+  }
   size = (o + 7u) & ~size_t(7);
 }
 
 bool HasDictionary(const std::vector<ColumnSlot>& slots) {
   for (const auto& s : slots)
     if (s.type.is_dict()) return true;
+  return false;
+}
+
+bool HasView(const std::vector<ColumnSlot>& slots) {
+  for (const auto& s : slots)
+    if (s.type.is_view()) return true;
   return false;
 }
 
@@ -322,8 +343,8 @@ struct KeyPlan {
 
 class BodyGen {
  public:
-  BodyGen(const Schema& schema, std::vector<ColumnSlot>* slots, bool nullable, bool coop)
-      : schema_(schema), slots_(slots), nullable_(nullable), coop_(coop) {}
+  BodyGen(const Schema& schema, std::vector<ColumnSlot>* slots, bool nullable, bool coop, bool view_sc = true)
+      : schema_(schema), slots_(slots), nullable_(nullable), coop_(coop), view_sc_(view_sc) {}
 
   // Device-scope definitions the body needs; GDV_NS = call sites that write text into scratch slots.
   std::string globals() const {
@@ -353,6 +374,7 @@ class BodyGen {
   const std::vector<CoopSeg>& coop_segs() const { return coop_segs_; }
   bool uses_ctx() const { return uses_ctx_; }
   const std::string& error() const { return error_; }
+  int view_shortcuts() const { return view_shortcuts_; }
 
   // Emit the statements that evaluate `node` for the row held in slot arrays at [k].
   Val Gen(const Node& node, std::string* out, int indent) {
@@ -714,8 +736,9 @@ class BodyGen {
   // which is what the cooperative LIKE scan needs.
   bool ViewChain(const Node& node, int* slot, unsigned* xf) {
     if (node.kind() == NodeKind::kField) {
-      // a dictionary column's rows are not one contiguous run of bytes
-      if (!node.return_type().is_varlen() || node.return_type().is_dict()) return false;
+      // a dictionary or view column's rows are not one contiguous run of bytes
+      const DataType& t = node.return_type();
+      if (!t.is_varlen() || t.is_dict() || t.is_view()) return false;
       *slot = SlotFor(static_cast<const FieldNode&>(node));
       *xf = 0u;
       return true;
@@ -931,6 +954,8 @@ class BodyGen {
     for (const auto& c : fn.children()) ptypes.push_back(c->return_type());
     const FunctionDef* def = Registry::Get().Lookup(fn.name(), ptypes);
     const DataType& rt = fn.return_type();
+
+    if (Val r; ViewShortcut(fn, out, indent, &r)) return r;
 
     if (def->flags & kDateFormat) {
       Val s = Gen(*fn.children()[0], out, indent);
@@ -1276,7 +1301,13 @@ class BodyGen {
     if (!c.parts.empty() && error_.empty()) error_ = "IN over concat(...) is not supported yet";
     const std::string v = NewVar("v");
     const DataType& t = n.value_type();
-    if (t.is_varlen()) {
+    if (const int j = ViewSlot(*n.child()); j >= 0 && t.is_varlen()) {
+      std::string e;
+      for (const auto& s : n.strs()) e += (e.empty() ? "" : " || ") + ViewTest(true, j, s);
+      if (e.empty()) e = "false";
+      ++view_shortcuts_;
+      *out += Ind(indent) + "const bool " + v + " = " + e + ";\n";
+    } else if (t.is_varlen()) {
       std::string e;
       std::vector<std::string> sorted = n.strs();
       std::sort(sorted.begin(), sorted.end());
@@ -1335,10 +1366,86 @@ class BodyGen {
     return Val{v, c.ok, boolean()};
   }
 
+  // ---- inline / prefix shortcut over string_view / binary_view columns (DESIGN.md §3.7) ----
+  // The slot of `node` when it is a bare view column and the shortcut is on, else -1.
+  int ViewSlot(const Node& node) {
+    if (!view_sc_ || node.kind() != NodeKind::kField || !node.return_type().is_view()) return -1;
+    return SlotFor(static_cast<const FieldNode&>(node));
+  }
+
+  // The test "the row of view slot j equals (equal) / starts with (!equal) the bytes b", decided from
+  // the raw view w<j>[k] in registers: the length first, then the inline bytes or the 4-byte prefix
+  // word; only out-of-line rows whose prefix agrees read their bytes, through the row's gdv_str.
+  std::string ViewTest(bool equal, int j, const std::string& b) {
+    uint32_t w[3] = {0u, 0u, 0u};
+    for (size_t i = 0; i < b.size() && i < 12; ++i)
+      w[i / 4] |= static_cast<uint32_t>(static_cast<uint8_t>(b[i])) << (8 * (i % 4));
+    const bool reads = equal ? b.size() > 12 : b.size() > 4;
+    const std::string arr = reads ? BytesArray(b, "gdv_lit_") : std::string("nullptr");
+    char words[64];
+    std::snprintf(words, sizeof(words), "0x%08xu, 0x%08xu, 0x%08xu", w[0], w[1], w[2]);
+    const std::string J = std::to_string(j);
+    return std::string(equal ? "gdv_sv_equal(" : "gdv_sv_starts(") + "w" + J + "[k], f" + J + "[k], " +
+           std::to_string(b.size()) + ", " + words + ", " + arr + ")";
+  }
+
+  // equal / not_equal / starts_with of a bare view column and a literal, and LIKE whose pattern
+  // starts with a literal run, lowered against the raw view (ViewTest).  string_scan bit 3 turns
+  // this off: the same calls then read the row's bytes through its gdv_str like any other function.
+  bool ViewShortcut(const FunctionNode& fn, std::string* out, int indent, Val* r) {
+    if (!view_sc_ || fn.children().size() < 2) return false;
+    const std::string& nm = fn.name();
+    const bool eq = nm == "equal" || nm == "not_equal";
+    if (!eq && nm != "starts_with" && nm != "like") return false;
+    const Node* col = fn.children()[0].get();
+    const Node* lit = fn.children()[1].get();
+    if (eq && col->kind() == NodeKind::kLiteral) std::swap(col, lit);
+    if (lit->kind() != NodeKind::kLiteral) return false;
+    const auto& l = static_cast<const LiteralNode&>(*lit);
+    if (l.is_null() || !l.return_type().is_varlen()) return false;
+    const int j = ViewSlot(*col);
+    if (j < 0) return false;
+    const Val c = Gen(*col, out, indent);
+    std::string test;
+    if (eq) {
+      test = (nm == "not_equal" ? "!" : "") + ViewTest(true, j, l.bytes());
+    } else if (nm == "starts_with") {
+      if (l.bytes().empty()) return false;
+      test = ViewTest(false, j, l.bytes());
+    } else {
+      const bool has_esc = fn.children().size() == 3;
+      const char esc = has_esc ? static_cast<const LiteralNode&>(*fn.children()[2]).bytes()[0] : 0;
+      const std::vector<unsigned> toks = LikeTokens(l.bytes(), has_esc, esc);
+      std::string head;
+      size_t i = 0;
+      for (; i < toks.size() && (toks[i] >> 8) == 0u; ++i) head.push_back(static_cast<char>(toks[i] & 0xffu));
+      if (head.empty()) return false;
+      if (i == toks.size()) {
+        test = ViewTest(true, j, head);  // no wildcard: the pattern is one string
+      } else if (i + 1 == toks.size() && (toks[i] >> 8) == 2u) {
+        test = ViewTest(false, j, head);  // 'lit%'
+      } else {
+        bool has_one = false;
+        for (unsigned t : toks) has_one = has_one || (t >> 8) == 1u;
+        const std::string match = has_one ? "gdv_like_match(" + c.v + ", " + LikePatternTable(toks) + ", " +
+                                                std::to_string(toks.size()) + ")"
+                                          : LikeSpecialised(toks) + "(" + c.v + ")";
+        test = ViewTest(false, j, head) + " && " + match;
+      }
+    }
+    ++view_shortcuts_;
+    const std::string v = NewVar("v");
+    *out += Ind(indent) + "const bool " + v + " = " + test + ";\n";
+    *r = Val{v, c.ok, boolean(), {}};
+    return true;
+  }
+
   const Schema& schema_;
   std::vector<ColumnSlot>* slots_;
   bool nullable_;
   bool coop_;
+  bool view_sc_;
+  int view_shortcuts_ = 0;
   std::string error_;  // first construct the fuser cannot lower (reported by GenerateKernel)
   std::vector<CoopSeg> coop_segs_;
   std::string globals_;
@@ -1378,6 +1485,10 @@ std::string EmitArgsStruct(const ArgsLayout& L) {
       << "  const u32* in_dvl[" << L.ni << "];  // validity words (or null),\n"
       << "  i64 in_dln[" << L.ni << "];         // length\n"
       << "  u32 in_dvs[" << L.ni << "];         // and validity bit shift; in_var = its bytes\n";
+  if (L.view)
+    s << "  const u8* const* in_vbf[" << L.ni << "];  // view columns: the data buffers' device pointers,\n"
+      << "  const i64* in_vsz[" << L.ni << "];        // their sizes\n"
+      << "  i64 in_vbn[" << L.ni << "];               // and count\n";
   s << "};\n";
   return s.str();
 }
@@ -1408,6 +1519,11 @@ void EmitPrologue(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, 
       *o += "  const u32* in_dvl" + J + " = A.in_dvl[" + J + "];\n";
       *o += "  const i64 in_dln" + J + " = A.in_dln[" + J + "];\n";
       *o += "  const u32 in_dvs" + J + " = A.in_dvs[" + J + "];\n";
+    } else if (t.is_view()) {
+      *o += "  const uint4* in_val" + J + " = reinterpret_cast<const uint4*>(A.in_val[" + J + "]);\n";
+      *o += "  const u8* const* in_vbf" + J + " = A.in_vbf[" + J + "];\n";
+      *o += "  const i64* in_vsz" + J + " = A.in_vsz[" + J + "];\n";
+      *o += "  const i64 in_vbn" + J + " = A.in_vbn[" + J + "];\n";
     } else if (t.is_varlen()) {
       *o += "  const i32* in_val" + J + " = reinterpret_cast<const i32*>(A.in_val[" + J + "]);\n";
       *o += "  const u8* in_var" + J + " = A.in_var[" + J + "];\n";
@@ -1592,9 +1708,15 @@ std::string DictView(const std::string& J, const std::string& ix) {
          ", &d" + J + "[k])";
 }
 
+// Row view of string_view / binary_view column J from its 16-byte view w<J>[k], loaded from `at`
+// (gdv_sv_view); the view's validity lands in d<J>[k].
+std::string SvView(const std::string& J, const std::string& at) {
+  return "gdv_sv_view(w" + J + "[k], " + at + ", in_vbf" + J + ", in_vsz" + J + ", in_vbn" + J + ", &d" + J + "[k])";
+}
+
 // A utf8 / binary column whose group of rows is one contiguous run of the data buffer (what the
-// shared-memory string stage copies); a dictionary column's rows are not.
-bool HasByteRun(const ColumnSlot& s) { return s.type.is_varlen() && !s.type.is_dict(); }
+// shared-memory string stage copies); a dictionary or view column's rows are not.
+bool HasByteRun(const ColumnSlot& s) { return s.type.is_varlen() && !s.type.is_dict() && !s.type.is_view(); }
 
 bool SlotHasCoop(const std::vector<CoopSeg>& segs, int j) {
   for (const auto& cs : segs)
@@ -1616,6 +1738,11 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
     if (spec.nullable) *o += I + "bool k" + std::to_string(j) + "[" + sR + "];\n";
     if (t.is_dict()) {
       // dictionary column: the entry behind the row's index is valid (and the index in range)
+      *o += I + "bool d" + std::to_string(j) + "[" + sR + "];\n";
+    } else if (t.is_view()) {
+      // view column: the raw 16-byte views (the inline / prefix shortcut reads them) and whether
+      // each view is valid
+      *o += I + "uint4 w" + std::to_string(j) + "[" + sR + "];\n";
       *o += I + "bool d" + std::to_string(j) + "[" + sR + "];\n";
     } else if (t.is_varlen()) {
       // group state of the string stage: rows known to be ASCII, cooperative-scan hit list usable
@@ -1647,10 +1774,11 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
       const std::string J = std::to_string(j);
       if (!t.is_bool())
         *o += I + "const " +
-              (t.is_dict() ? std::string(DataType(t.index).ctype())
-                           : t.is_varlen() ? std::string("i32") : std::string(t.ctype())) +
+              (t.is_dict()   ? std::string(DataType(t.index).ctype())
+               : t.is_view() ? std::string("uint4")
+               : t.is_varlen() ? std::string("i32") : std::string(t.ctype())) +
               "* ptr" + J + " = in_val" + J + " + base + (i64)lane;\n";
-      if (t.is_varlen() && !t.is_dict() && stage_bytes > 0) {
+      if (HasByteRun(slots[j]) && stage_bytes > 0) {
         // The bytes of the group's 32*R strings are one contiguous run: copy it into this
         // warp's shared-memory stage with coalesced 16-byte loads, then every lane walks its
         // own string out of shared memory instead of issuing one global load per byte.
@@ -1710,6 +1838,9 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
               ") >> lane) & 1u) != 0u;\n";
       } else if (t.is_dict()) {
         *o += I + "  f" + J + "[k] = " + DictView(J, "(i64)gdv_ldp(ptr" + J + " + 32 * k)") + ";\n";
+      } else if (t.is_view()) {
+        *o += I + "  w" + J + "[k] = gdv_ldview(ptr" + J + " + 32 * k);\n";
+        *o += I + "  f" + J + "[k] = " + SvView(J, "ptr" + J + " + 32 * k") + ";\n";
       } else if (t.is_varlen()) {
         *o += I + "  { const i32 sb = ptr" + J + "[32 * k]; const i32 se = ptr" + J +
               "[32 * k + 1]; f" + J + "[k] = gdv_make_str(" +
@@ -1729,7 +1860,8 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
           *o += I + "  k" + J + "[k] = true;\n";
         else
           *o += I + "  k" + J + "[k] = ((gdv_ldwin(in_vp" + J + ", ((base >> 5) + k) & in_vm" + J + ", in_vsh" +
-                J + ") >> lane) & 1u) != 0u" + (slots[j].type.is_dict() ? " && d" + J + "[k]" : "") + ";\n";
+                J + ") >> lane) & 1u) != 0u" +
+                (slots[j].type.is_dict() || slots[j].type.is_view() ? " && d" + J + "[k]" : "") + ";\n";
       }
       *o += I + "}\n";
     }
@@ -1747,6 +1879,9 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
               J + ", r);\n";
       } else if (t.is_dict()) {
         *o += I + "  f" + J + "[k] = " + DictView(J, "in ? (i64)gdv_ldp(in_val" + J + " + r) : -1ll") + ";\n";
+      } else if (t.is_view()) {
+        *o += I + "  w" + J + "[k] = in ? gdv_ldview(in_val" + J + " + r) : make_uint4(0u, 0u, 0u, 0u);\n";
+        *o += I + "  f" + J + "[k] = " + SvView(J, "in_val" + J + " + r") + ";\n";
       } else if (t.is_varlen()) {
         *o += I + "  { const i32 sb = in ? in_val" + J + "[r] : 0; const i32 se = in ? in_val" + J +
               "[r + 1] : 0; f" + J + "[k] = gdv_make_str(in_var" + J + " + sb, se - sb); }\n";
@@ -1757,7 +1892,7 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
         *o += I + "  k" + J + "[k] = in;\n";
       else if (spec.nullable)
         *o += I + "  k" + J + "[k] = in && (!in_hv" + J + " || gdv_ldbit(reinterpret_cast<const u8*>(in_vld" +
-              J + "), in_vsh" + J + ", r))" + (t.is_dict() ? " && d" + J + "[k]" : "") + ";\n";
+              J + "), in_vsh" + J + ", r))" + (t.is_dict() || t.is_view() ? " && d" + J + "[k]" : "") + ";\n";
     }
     *o += I + "}\n";
   }
@@ -1770,7 +1905,7 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
   *o += I + "}\n";
   if (fast && stage_bytes > 0) {
     bool any = false;
-    for (const auto& sl : slots) any = any || sl.type.is_varlen();
+    for (const auto& sl : slots) any = any || (sl.type.is_varlen() && !sl.type.is_view());
     if (any) *o += I + "__syncwarp();  // all lanes are done with the stage before it is refilled\n";
   }
 }
@@ -2218,8 +2353,8 @@ void ApplyDeviceCount(std::string* src) {
 void MarkHoisted(const BodyGen& gen, const Node& cond, std::vector<ColumnSlot>* slots) {
   std::vector<int> strict;
   gen.TruthStrict(cond, &strict);
-  for (auto& sl : *slots)  // a dictionary row's validity also depends on its entry: read per row
-    if (!sl.type.is_dict() && std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end())
+  for (auto& sl : *slots)  // a dictionary / view row's validity also depends on its entry / view: read per row
+    if (!sl.type.is_dict() && !sl.type.is_view() && std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end())
       sl.hoist = true;
 }
 
@@ -2249,14 +2384,14 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
                             GeneratedKernel* out) {
   const bool is_size = spec.kind == KernelKind::kStringSize;
   std::vector<ColumnSlot> slots;
-  BodyGen gen(schema, &slots, spec.nullable, (spec.string_scan & 1) == 0);
+  BodyGen gen(schema, &slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
   std::string body;
   const Val res = gen.Gen(*expr->root(), &body, 4);
   if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
   int n_varlen = 0, in_bytes = 0;
   for (const auto& s : slots) {
     n_varlen += HasByteRun(s) ? 1 : 0;
-    in_bytes += s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);
+    in_bytes += s.type.is_view() ? 16 : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);
   }
   int R = spec.rows_per_thread > 0 ? std::min(spec.rows_per_thread, 8) : 2;
   // String predicates are instruction-bound and stage bytes per warp in shared memory: they run
@@ -2282,7 +2417,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   const int col_block = stage_bytes + hit_bytes;
   const int dynamic_smem = col_block * NW * n_varlen;
   const bool has_sel = spec.selection_mode != GDV_SEL_NONE;
-  ArgsLayout L(static_cast<int>(slots.size()), 1, HasDictionary(slots));
+  ArgsLayout L(static_cast<int>(slots.size()), 1, HasDictionary(slots), HasView(slots));
   const std::string sR = std::to_string(R), s32R = std::to_string(32 * R), sT = std::to_string(T);
 
   std::string src;
@@ -2451,6 +2586,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   out->staged = false;
   out->stages = 0;
   out->cta_tile_rows = T;
+  out->view_shortcuts = gen.view_shortcuts();
   return Status::OK();
 }
 
@@ -2616,7 +2752,7 @@ NodePtr WithValueTypes(const NodePtr& node) {
 
 static bool ReadsDictionary(const Node& node) {
   switch (node.kind()) {
-    case NodeKind::kField: return node.return_type().is_dict();
+    case NodeKind::kField: return node.return_type().is_dict() || node.return_type().is_view();
     case NodeKind::kLiteral: return false;
     case NodeKind::kFunction:
       for (const auto& c : static_cast<const FunctionNode&>(node).children())
@@ -2642,8 +2778,8 @@ Status GenerateKernel(const Schema& schema, const std::vector<ExpressionPtr>& ex
   for (const auto& e : exprs) {
     NodePtr r = RewriteAliases(e->root());
     lowered.push_back(r == e->root() ? e : std::make_shared<Expression>(r, e->result()));
-    // a dictionary row is null when its entry is, or when its index is out of range: such kernels
-    // always keep the validity plumbing
+    // a dictionary row is null when its entry is, or when its index is out of range, and a view row
+    // when its view is invalid: such kernels always keep the validity plumbing
     if (ReadsDictionary(*r)) s.nullable = true;
   }
   return GenerateKernelImpl(schema, lowered, s, out);
@@ -2674,7 +2810,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
       std::string kbody;
       const Val kres = kgen.GenTruth(*exprs[0]->root(), &kbody, 6);
       // the anchor drain loads rows one by one from plain columns only
-      if (kgen.error().empty() && !kgen.uses_ctx() && !HasDictionary(kslots)) {
+      if (kgen.error().empty() && !kgen.uses_ctx() && !HasDictionary(kslots) && !HasView(kslots)) {
         if (spec.nullable) MarkHoisted(kgen, *exprs[0]->root(), &kslots);
         ArgsLayout KL(static_cast<int>(kslots.size()), 0);
         std::string src = "// generated by gandiva_b200 kernel fuser; key-driven string Filter";
@@ -2712,7 +2848,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
     }
   }
   std::vector<ColumnSlot> slots;
-  BodyGen gen(schema, &slots, spec.nullable, (spec.string_scan & 1) == 0);
+  BodyGen gen(schema, &slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
 
   // Per-row body (uses f<j>[k] / k<j>[k]); generated first so we know the slots.
   std::string body;
@@ -2733,6 +2869,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   int n_varlen = 0;
   for (const auto& s : slots) {
     in_bytes += s.type.is_dict() ? DataType(s.type.index).width()  // the index; the dictionary is cached
+                : s.type.is_view()   ? 16                               // the view; out-of-line bytes on demand
                 : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);  // 4 B offset + ~28 B data
     n_varlen += HasByteRun(s) ? 1 : 0;
   }
@@ -2821,7 +2958,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
       dynamic_smem = S * stage_total;
     }
   }
-  ArgsLayout L(static_cast<int>(slots.size()), n_out, HasDictionary(slots));
+  ArgsLayout L(static_cast<int>(slots.size()), n_out, HasDictionary(slots), HasView(slots));
 
   std::string src;
   src += "// generated by gandiva_b200 kernel fuser; one fused kernel per ";
@@ -2840,7 +2977,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   bool light = spec.kind == KernelKind::kFilter && n_varlen == 0 && BT >= 256 && 2048 % BT == 0 &&
                !gen.uses_ctx() && body.size() < 6000;
   for (const auto& sl : slots)  // 128-bit math and string functions over dictionary views want registers
-    light = light && !sl.type.is_decimal() && !sl.type.is_dict();
+    light = light && !sl.type.is_decimal() && !sl.type.is_dict() && !sl.type.is_view();
   if (W > 1) light = false;  // W chunks keep 2 W more registers
   if (light) bounds += ", " + std::to_string(2048 / BT);
   src += "extern \"C\" __global__ void __launch_bounds__(" + bounds + ") " + spec.name +
@@ -3144,6 +3281,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   out->staged = staged;
   out->stages = staged ? S : 0;
   out->cta_tile_rows = static_cast<int64_t>(BT) * R;
+  out->view_shortcuts = gen.view_shortcuts();
   return Status::OK();
 }
 

@@ -46,6 +46,7 @@ struct KernelSpec {
                                       // fixed-width filter: 1024-row chunks every warp walks per tile (1/2/4/8)
   int string_scan = 0;                // bit 0: LIKE with the per-lane matcher only (no cooperative scan);
                                       // bit 2: row-driven string filter even where the key-driven one applies
+                                      // bit 3: no inline / prefix shortcut over string_view / binary_view views
 };
 
 struct ColumnSlot {
@@ -77,6 +78,7 @@ struct GeneratedKernel {
   bool staged = false;              // project: inputs staged through shared memory by TMA bulk copies
   int stages = 0;                   // staged: shared-memory stages per CTA
   int64_t cta_tile_rows = 0;        // staged: rows per CTA tile (block_threads * rows_per_thread)
+  int view_shortcuts = 0;           // call sites decided from the raw 16-byte views (BodyGen::ViewShortcut)
 };
 
 // Byte offsets inside gdv_args; the host packs the same layout (see EmitArgsStruct()).
@@ -90,10 +92,16 @@ struct ArgsLayout {
   // dictionary's offsets, validity word pointer, length and validity bit shift.  Zero otherwise.
   bool dict = false;
   size_t off_in_dof = 0, off_in_dvl = 0, off_in_dln = 0, off_in_dvs = 0;
-  ArgsLayout(int n_inputs, int n_outputs, bool dictionary = false);
+  // Kernels that read a string_view / binary_view column get one more block per input (HasView):
+  // the device pointer of the data buffers' pointer table, the sizes' device pointer and the buffer
+  // count.  Zero otherwise, so every other kernel keeps its layout and source.
+  bool view = false;
+  size_t off_in_vbf = 0, off_in_vsz = 0, off_in_vbn = 0;
+  ArgsLayout(int n_inputs, int n_outputs, bool dictionary = false, bool views = false);
 };
 
 bool HasDictionary(const std::vector<ColumnSlot>& slots);
+bool HasView(const std::vector<ColumnSlot>& slots);
 
 Status GenerateKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs,
                       const KernelSpec& spec, GeneratedKernel* out);

@@ -30,6 +30,7 @@ static const char* unit_name(int u) {
 }
 
 std::string DataType::ToString() const {
+  if (view) return id == GDV_TYPE_BINARY ? "binary_view" : "string_view";
   if (index != 0)
     return "dictionary<values=" + value_type().ToString() + ", indices=" + DataType(index).ToString() +
            ", ordered=" + (ordered ? "1" : "0") + ">";

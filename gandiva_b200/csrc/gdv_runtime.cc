@@ -426,13 +426,16 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
 
 // One kernel input after staging: device addresses + bit shifts.  Dictionary columns: val / vld /
 // vsh are the indices', var the dictionary's bytes, and dof / dvl / dvs / dln the dictionary's
-// offsets, validity words, bit shift and length.
+// offsets, validity words, bit shift and length.  View columns: val is the views, and vbf / vsz /
+// vbn the device pointer table of the data buffers, their sizes and their count.
 struct ResolvedIn {
   CUdeviceptr val = 0, vld = 0, var = 0;
   uint32_t vsh = 0, dsh = 0;
   CUdeviceptr dof = 0, dvl = 0;
   uint32_t dvs = 0;
   int64_t dln = 0;
+  CUdeviceptr vbf = 0, vsz = 0;
+  int64_t vbn = 0;
 };
 
 inline int64_t BitBytes(int64_t bit_begin, int64_t nbits) {
@@ -488,6 +491,45 @@ Status ResolveDictionary(Device* dev, int col, const gdv_column_t& c, bool host,
   if (vbytes > 0)
     GDV_RETURN_NOT_OK(StagedHtoD(dev, dv, static_cast<const uint8_t*>(dict->data) + first, vbytes, stream));
   r->var = dv - static_cast<CUdeviceptr>(first);  // kernel addresses bytes as var + offs[i]
+  return Status::OK();
+}
+
+// The data buffers of a string_view / binary_view column (gdv_view_buffers_t, reached through
+// var_data).  Device batches: the buffers and their sizes are read in place; only the host array of
+// buffer pointers is copied, asynchronously on `stream`, into pooled scratch.  Host batches: every
+// buffer is staged whole (a sliced batch may carry bytes no row of the slice uses), and the table of
+// their device copies and the sizes next to them.  Only what is cheap is checked here; a view that
+// reaches outside its buffer is caught per row by the kernel (gdv_sv_view).
+Status ResolveViewBuffers(Device* dev, int col, const gdv_column_t& c, bool host, CUstream stream,
+                          ScratchScope* scratch, ResolvedIn* r) {
+  const auto* vb = static_cast<const gdv_view_buffers_t*>(c.var_data);
+  const std::string what = "view column " + std::to_string(col);
+  if (vb == nullptr)
+    return Status::Make(GDV_INVALID, what + " has no data buffers (var_data must point at a gdv_view_buffers_t)");
+  if (vb->n < 0) return Status::Make(GDV_INVALID, what + ": negative data buffer count");
+  r->vbn = vb->n;
+  if (vb->n == 0) return Status::OK();  // every valid view is inline
+  if (vb->data == nullptr || vb->sizes == nullptr)
+    return Status::Make(GDV_INVALID, what + ": null data buffer table or sizes");
+  const size_t tbytes = static_cast<size_t>(vb->n) * 8;
+  GDV_RETURN_NOT_OK(scratch->Alloc(tbytes, &r->vbf));
+  if (!host) {
+    GDV_RETURN_NOT_OK(StagedHtoD(dev, r->vbf, vb->data, tbytes, stream));
+    r->vsz = reinterpret_cast<CUdeviceptr>(vb->sizes);
+    return Status::OK();
+  }
+  std::vector<CUdeviceptr> table(static_cast<size_t>(vb->n), 0);
+  for (int32_t i = 0; i < vb->n; ++i) {
+    const int64_t sz = vb->sizes[i];
+    if (sz < 0) return Status::Make(GDV_INVALID, what + ": negative size of data buffer " + std::to_string(i));
+    if (sz == 0) continue;
+    if (vb->data[i] == nullptr) return Status::Make(GDV_INVALID, what + ": data buffer " + std::to_string(i) + " is null");
+    GDV_RETURN_NOT_OK(scratch->Alloc(static_cast<size_t>(sz) + 16, &table[static_cast<size_t>(i)]));
+    GDV_RETURN_NOT_OK(StagedHtoD(dev, table[static_cast<size_t>(i)], vb->data[i], static_cast<size_t>(sz), stream));
+  }
+  GDV_RETURN_NOT_OK(StagedHtoD(dev, r->vbf, table.data(), tbytes, stream));
+  GDV_RETURN_NOT_OK(scratch->Alloc(tbytes, &r->vsz));
+  GDV_RETURN_NOT_OK(StagedHtoD(dev, r->vsz, vb->sizes, tbytes, stream));
   return Status::OK();
 }
 
@@ -556,6 +598,22 @@ Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t*
         r.val = reinterpret_cast<CUdeviceptr>(p);
       }
       GDV_RETURN_NOT_OK(ResolveDictionary(dev, slot.schema_index, c, host, stream, scratch, &r));
+    } else if (t.is_view()) {
+      // the 16-byte views like a fixed-width column, then the data buffers
+      const uint8_t* p = static_cast<const uint8_t*>(c.values) + off * 16;
+      if (host) {
+        const size_t bytes = static_cast<size_t>(n) * 16;
+        CUdeviceptr dp;
+        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 16, &dp));
+        if (bytes > 0) GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
+        r.val = dp;
+      } else {
+        if (reinterpret_cast<uintptr_t>(p) % 16u != 0)
+          return Status::Make(GDV_INVALID, "device views buffer of column " + std::to_string(slot.schema_index) +
+                                               " is not 16-byte aligned");
+        r.val = reinterpret_cast<CUdeviceptr>(p);
+      }
+      GDV_RETURN_NOT_OK(ResolveViewBuffers(dev, slot.schema_index, c, host, stream, scratch, &r));
     } else if (t.is_varlen()) {
       const int32_t* offs = static_cast<const int32_t*>(c.values) + off;
       if (host) {
@@ -616,6 +674,11 @@ void PutInputs(std::vector<uint8_t>& args, const ArgsLayout& L, const std::vecto
       Put<CUdeviceptr>(args, L.off_in_dvl + 8 * j, ins[j].dvl);
       Put<int64_t>(args, L.off_in_dln + 8 * j, ins[j].dln);
       Put<uint32_t>(args, L.off_in_dvs + 4 * j, ins[j].dvs);
+    }
+    if (L.view) {
+      Put<CUdeviceptr>(args, L.off_in_vbf + 8 * j, ins[j].vbf);
+      Put<CUdeviceptr>(args, L.off_in_vsz + 8 * j, ins[j].vsz);
+      Put<int64_t>(args, L.off_in_vbn + 8 * j, ins[j].vbn);
     }
   }
 }
@@ -860,11 +923,11 @@ Status Projector::KernelFor(bool nullable, CompiledKernel** out) {
   return Status::OK();
 }
 
-// True when some column the kernel reads carries a validity bitmap, or is dictionary-encoded (a
-// row is also null where its dictionary entry is).
+// True when some column the kernel reads carries a validity bitmap, or is dictionary-encoded or a
+// view column (a row is also null where its dictionary entry is, or where its view is invalid).
 static bool AnyValidity(const GeneratedKernel& gen, const gdv_batch_t* batch) {
   for (const auto& slot : gen.inputs)
-    if (slot.type.is_dict() || (slot.schema_index >= 0 && slot.schema_index < batch->num_columns &&
+    if (slot.type.is_dict() || slot.type.is_view() || (slot.schema_index >= 0 && slot.schema_index < batch->num_columns &&
                                 batch->columns[slot.schema_index].validity != nullptr))
       return true;
   return false;
@@ -954,7 +1017,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   scratch.Guard(stream);
   std::vector<ResolvedIn> ins;
   GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), 1, HasDictionary(gen.inputs));
+  ArgsLayout L(static_cast<int>(gen.inputs.size()), 1, HasDictionary(gen.inputs), HasView(gen.inputs));
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
   PutInputs(args, L, ins);
@@ -1112,7 +1175,7 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
   GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
   const double t_inputs = TraceOn() ? NowUs() : 0.0;
 
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), n_outs, HasDictionary(gen.inputs));
+  ArgsLayout L(static_cast<int>(gen.inputs.size()), n_outs, HasDictionary(gen.inputs), HasView(gen.inputs));
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
   PutInputs(args, L, ins);
@@ -1498,7 +1561,7 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
                                             out_sel->index_base, bounded ? out_sel->max_slots : n, &scratch));
   } else {
     const GeneratedKernel& gen = kernel->gen;
-    ArgsLayout L(static_cast<int>(gen.inputs.size()), 0, HasDictionary(gen.inputs));
+    ArgsLayout L(static_cast<int>(gen.inputs.size()), 0, HasDictionary(gen.inputs), HasView(gen.inputs));
     std::vector<uint8_t> args(L.size, 0);
     Put<int64_t>(args, L.off_n, n);
     Put<int64_t>(args, L.off_row_base, out_sel->index_base);

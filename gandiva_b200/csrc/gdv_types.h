@@ -13,12 +13,17 @@ namespace gdv {
 // Everything that reads values -- function resolution, if/else and IN type checks -- sees the
 // value type; operator== compares value types, same() also the encoding.  At the C-ABI it is
 // GDV_TYPE_DICTIONARY (include/gandiva_b200.h).
+// A string_view / binary_view column (arrow::StringViewType / BinaryViewType) works the same way:
+// `id` is GDV_TYPE_STRING / BINARY and `view` is set, so everything that reads values sees utf8 /
+// binary and only same() and the kernels' row loaders see the 16-byte views.  is_varlen() holds
+// for all three layouts; HasByteRun (gdv_codegen.cc) is what "contiguous offsets + bytes" means.
 struct DataType {
   int32_t id = GDV_TYPE_NA;
   int32_t precision = 0;  // decimal precision, or time unit for timestamp/time
   int32_t scale = 0;
   int32_t index = 0;      // dictionary columns: GDV_TYPE_INT8..INT64 (or what the caller sent)
   bool ordered = false;   // dictionary columns: DictionaryType::ordered
+  bool view = false;      // string_view / binary_view columns
 
   DataType() = default;
   DataType(int32_t i, int32_t p = 0, int32_t s = 0) : id(i), precision(p), scale(s) {}
@@ -28,16 +33,24 @@ struct DataType {
       index = t.precision & 0xff;
       ordered = (t.precision & GDV_DICT_ORDERED) != 0;
       precision = scale = 0;
+    } else if (t.id == GDV_TYPE_STRING_VIEW || t.id == GDV_TYPE_BINARY_VIEW) {
+      id = t.id == GDV_TYPE_STRING_VIEW ? GDV_TYPE_STRING : GDV_TYPE_BINARY;
+      view = true;
+      precision = scale = 0;
     }
   }
   gdv_type_t c() const {
+    if (view) return gdv_type_t{id == GDV_TYPE_BINARY ? GDV_TYPE_BINARY_VIEW : GDV_TYPE_STRING_VIEW, 0, 0};
     if (index != 0) return gdv_type_t{GDV_TYPE_DICTIONARY, index | (ordered ? GDV_DICT_ORDERED : 0), id};
     return gdv_type_t{id, precision, scale};
   }
   bool is_dict() const { return index != 0; }
-  // The type of the values (the dictionary's type for a dictionary column).
+  bool is_view() const { return view; }
+  // The type of the values (the dictionary's type for a dictionary column, utf8 / binary for a view).
   DataType value_type() const { return DataType(id, precision, scale); }
-  bool same(const DataType& o) const { return *this == o && index == o.index && ordered == o.ordered; }
+  bool same(const DataType& o) const {
+    return *this == o && index == o.index && ordered == o.ordered && view == o.view;
+  }
 
   bool operator==(const DataType& o) const {
     if (id != o.id) return false;

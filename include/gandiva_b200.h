@@ -90,6 +90,12 @@ typedef int32_t gdv_status;
  * dictionary result type, is refused at Make() with GDV_NOT_IMPLEMENTED. */
 #define GDV_TYPE_DICTIONARY 29
 #define GDV_DICT_ORDERED 0x100
+/* Arrow's 16-byte view layouts of utf8 / binary (arrow::StringViewType, BinaryViewType; C format
+ * "vu" / "vz"), described by gdv_view_buffers_t.  Input columns only, like dictionary columns:
+ * functions resolve against utf8 / binary, and results are plain utf8 / binary.  A view result
+ * type is refused at Make() with GDV_NOT_IMPLEMENTED. */
+#define GDV_TYPE_STRING_VIEW 39
+#define GDV_TYPE_BINARY_VIEW 40
 
 typedef struct gdv_type {
   int32_t id;        /* GDV_TYPE_* */
@@ -124,7 +130,10 @@ typedef struct gdv_config {
                               bit 0: LIKE with the per-lane matcher only (no warp-cooperative scan),
                               bit 2: row-driven string Filter kernel even where the condition implies a
                                      literal and the key-driven kernel (driven by the literal's
-                                     occurrences in the column's bytes) would apply */
+                                     occurrences in the column's bytes) would apply,
+                              bit 3 (value 8): string_view / binary_view columns: no inline / prefix
+                                     shortcut; equal, IN, starts_with and LIKE 'lit%...' read the row's
+                                     bytes through the view like any other string function */
   int32_t reserved[3];
 } gdv_config_t;
 void gdv_config_default(gdv_config_t* cfg);
@@ -148,6 +157,7 @@ void gdv_config_default(gdv_config_t* cfg);
  *  fixed width : validity | values                (values = buffers[1])
  *  bool        : validity | bit-packed values
  *  utf8/binary : validity | int32 offsets | bytes (values = offsets, var_data = bytes)
+ *  string_view / binary_view : validity | 16-byte views | var_data = gdv_view_buffers_t* (below)
  * `offset` is ArrayData::offset (in elements/bits), applied to every buffer.
  * validity may be NULL (no nulls). */
 typedef struct gdv_column {
@@ -176,6 +186,23 @@ typedef struct gdv_dictionary {
   int64_t length;        /* entries */
   int64_t data_size;     /* bytes in data (needed to stage host dictionaries) */
 } gdv_dictionary_t;
+
+/* The data buffers of a string_view / binary_view column (GDV_TYPE_STRING_VIEW / BINARY_VIEW).
+ * The column itself is
+ *  view        : validity | 16-byte views (values) | var_data = const gdv_view_buffers_t*
+ * with `offset` applying to the validity and the views.  A view is {int32 len, then either the
+ * len <= 12 bytes inline (zero padded), or a 4-byte prefix, int32 buffer index and int32 offset into
+ * data[buffer index]}.  A non-null view is invalid Arrow input when len < 0, or when len > 12 and the
+ * buffer index is outside [0, n), the offset is negative or offset + len > sizes[buffer index]: its
+ * row reads as null and nothing is dereferenced for it.  Null slots are never read through.  Host
+ * batches stage the validity, the views and every data buffer whole (a sliced batch may carry bytes
+ * no row in the slice uses); device batches read them in place.  The struct is read during the
+ * Evaluate call only. */
+typedef struct gdv_view_buffers {
+  const void* const* data; /* host array of n buffer pointers, in the batch's memory space */
+  const int64_t* sizes;    /* n byte sizes, in the batch's memory space */
+  int32_t n;               /* data buffers (may be 0: every view is inline) */
+} gdv_view_buffers_t;
 
 typedef struct gdv_batch {
   int64_t num_rows;
@@ -281,7 +308,8 @@ gdv_status gdv_projector_kernel_info(gdv_projector_t p, char* name_buf, int64_t 
                                      int32_t* block_threads);
 /* Integer attribute of the kernel variant used by the latest Evaluate: "staged" (1 = TMA bulk
  * loader), "stages", "dynamic_smem", "cta_tile_rows", "tile_rows", "nullable",
- * "in_bytes_per_row", "blocks_per_sm" (needs a device). */
+ * "in_bytes_per_row", "view_shortcuts" (call sites decided from the 16-byte views of string_view /
+ * binary_view columns: equal, IN, starts_with, LIKE 'lit%...'), "blocks_per_sm" (needs a device). */
 gdv_status gdv_projector_kernel_attr(gdv_projector_t p, const char* key, int64_t* out);
 void gdv_projector_release(gdv_projector_t p);
 
