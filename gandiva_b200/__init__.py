@@ -66,7 +66,7 @@ class gdv_config_t(C.Structure):
     _fields_ = [("optimize", C.c_int32), ("dump_ir", C.c_int32), ("device", C.c_int32),
                 ("rows_per_thread", C.c_int32), ("block_threads", C.c_int32),
                 ("loader", C.c_int32), ("sm_reserve", C.c_int32), ("stages", C.c_int32),
-                ("string_scan", C.c_int32), ("reserved", C.c_int32 * 3)]
+                ("string_scan", C.c_int32), ("filter_gating", C.c_int32), ("reserved", C.c_int32 * 2)]
 
 
 class gdv_column_t(C.Structure):
@@ -512,9 +512,10 @@ class Configuration:
 
     def __init__(self, optimize: bool = True, dump_ir: bool = False, device: int = 0,
                  rows_per_thread: int = 0, block_threads: int = 0, loader: int = 0,
-                 sm_reserve: int = 0, stages: int = 0, string_scan: int = 0):
+                 sm_reserve: int = 0, stages: int = 0, string_scan: int = 0, filter_gating: int = 0):
         self.stages = int(stages)
         self.string_scan = int(string_scan)
+        self.filter_gating = int(filter_gating)
         self.optimize = bool(optimize)
         self.dump_ir = bool(dump_ir)
         self.device = int(device)
@@ -535,6 +536,7 @@ class Configuration:
         c.sm_reserve = self.sm_reserve
         c.stages = self.stages
         c.string_scan = self.string_scan
+        c.filter_gating = self.filter_gating
         return c
 
 
@@ -690,7 +692,7 @@ def _kernel_info(fn, handle, attr_fn=None) -> dict:
         keys = ["staged", "stages", "dynamic_smem", "cta_tile_rows", "tile_rows", "nullable"]
         keys.append("view_shortcuts")
         if attr_fn is lib.gdv_filter_kernel_attr:
-            keys.append("dictionary_first")
+            keys += ["dictionary_first", "gated_stages"]
         if regs.value >= 0:
             keys.append("blocks_per_sm")
         for key in keys:

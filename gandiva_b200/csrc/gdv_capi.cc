@@ -54,6 +54,7 @@ Config FromC(const gdv_config_t* c) {
     cfg.loader = c->loader;
     cfg.stages = c->stages;
     cfg.string_scan = c->string_scan;
+    cfg.filter_gating = c->filter_gating;
     cfg.sm_reserve = c->sm_reserve;
   }
   return cfg;
@@ -320,6 +321,7 @@ static gdv_status KernelAttr(CompiledKernel& k, const Config& cfg, const char* k
   if (kk == "nullable") { *out = k.gen.nullable ? 1 : 0; return GDV_OK; }
   if (kk == "in_bytes_per_row") { *out = k.gen.in_bytes_per_row; return GDV_OK; }
   if (kk == "view_shortcuts") { *out = k.gen.view_shortcuts; return GDV_OK; }
+  if (kk == "gated_stages") { *out = k.gen.gated_stages; return GDV_OK; }
   if (kk == "blocks_per_sm") {
     Device* dev = nullptr;
     Status s = Device::Get(cfg.device, &dev);

@@ -1910,6 +1910,102 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int
   }
 }
 
+// Gated loads of a fixed-width Filter (DESIGN.md §3.3): the conjuncts of the condition's AND spine
+// are evaluated in stages, and stage s loads its columns only in the rows every earlier stage kept.
+// Stage s loads slots [first_slot[s], first_slot[s + 1]) (slots are numbered by first appearance on
+// the spine) and ANDs in the conjuncts whose last column is among them (PlanGate).
+struct GatePlan {
+  std::vector<int> first_slot;                      // one per stage, plus slots.size() at the end
+  std::vector<std::vector<const Node*>> conjuncts;  // per stage, in spine order
+  int stages() const { return static_cast<int>(conjuncts.size()); }
+};
+
+// One group of R steps of a gated fixed-width Filter (GatePlan; mode kFast or kPred).  Stage 0 loads
+// like EmitGroup; the loads of a later stage are issued, all R of them, only in the lanes whose row
+// is still alive, so a row that an earlier conjunct dropped reads none of the later columns' bytes.
+// A group in which stage 0 kept every row loads all later columns at once instead.
+// seg[s] evaluates stage s's conjuncts for row [k] and ANDs them into alive[k]; validity (per-row or
+// hoisted) is read as EmitGroup reads it, whatever the stage.
+void EmitGatedGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int R, int mode,
+                    const GatePlan& plan, const std::vector<std::string>& seg, const std::string& step_tail,
+                    std::string* o, int indent) {
+  const bool fast = mode == kFast;
+  const std::string I(static_cast<size_t>(indent) * 2, ' ');
+  const std::string sR = std::to_string(R);
+  for (size_t j = 0; j < slots.size(); ++j) {
+    *o += I + slots[j].type.ctype() + " f" + std::to_string(j) + "[" + sR + "];\n";
+    if (spec.nullable) *o += I + "bool k" + std::to_string(j) + "[" + sR + "];\n";
+  }
+  *o += I + "bool alive[" + sR + "];\n";
+  if (fast)
+    for (size_t j = 0; j < slots.size(); ++j)
+      *o += I + "const " + slots[j].type.ctype() + "* ptr" + std::to_string(j) + " = in_val" + std::to_string(j) +
+            " + base + (i64)lane;\n";
+  const std::string row = I + "  const i64 s = base + 32 * k + (i64)lane;\n" +
+                          I + (fast ? "  const bool in = true;\n" : "  const bool in = s < A.n;\n");
+  // stage st: its loads (stage 0: the validity of every column too; `dense`: unpredicated), then its conjuncts
+  auto stage = [&](int st, bool load, bool dense, const std::string& J2) {
+    if (load) {
+      *o += J2 + "#pragma unroll\n";
+      *o += J2 + "for (int k = 0; k < " + sR + "; ++k) {\n";
+      if (!fast || (st == 0 && spec.nullable)) *o += row;
+      const std::string on = st == 0 ? std::string("in") : std::string("alive[k]");
+      const int last = dense ? static_cast<int>(slots.size()) : plan.first_slot[st + 1];
+      for (int j = plan.first_slot[st]; j < last; ++j) {
+        const std::string J = std::to_string(j);
+        const std::string zero = std::string("(") + slots[j].type.ctype() + ")0";
+        if (fast && (st == 0 || dense))
+          *o += J2 + "  f" + J + "[k] = gdv_ldp(ptr" + J + " + 32 * k);\n";
+        else if (fast)
+          *o += J2 + "  f" + J + "[k] = alive[k] ? gdv_ldp(ptr" + J + " + 32 * k) : " + zero + ";\n";
+        else
+          *o += J2 + "  f" + J + "[k] = " + on + " ? gdv_ldp(in_val" + J + " + s) : " + zero + ";\n";
+      }
+      if (st == 0 && spec.nullable) {
+        for (size_t j = 0; j < slots.size(); ++j) {
+          const std::string J = std::to_string(j);
+          if (slots[j].hoist)  // validity ANDed into the keep-mask after the row loop (EmitFilterEpilogue)
+            *o += J2 + "  k" + J + "[k] = in;\n";
+          else if (fast)
+            *o += J2 + "  k" + J + "[k] = ((gdv_ldwin(in_vp" + J + ", ((base >> 5) + k) & in_vm" + J + ", in_vsh" + J +
+                  ") >> lane) & 1u) != 0u;\n";
+          else
+            *o += J2 + "  k" + J + "[k] = in && (!in_hv" + J + " || gdv_ldbit(reinterpret_cast<const u8*>(in_vld" + J +
+                  "), in_vsh" + J + ", s));\n";
+        }
+      }
+      *o += J2 + "}\n";
+    }
+    *o += J2 + "#pragma unroll\n";
+    *o += J2 + "for (int k = 0; k < " + sR + "; ++k) {\n";
+    *o += row;
+    if (st == 0) *o += J2 + "  alive[k] = in;\n";
+    *o += seg[static_cast<size_t>(st)];
+    *o += J2 + "}\n";
+  };
+  stage(0, true, false, I);
+  if (fast && plan.stages() > 2) {
+    // Every row of the group survived stage 0 (a condition whose first conjuncts keep most rows):
+    // gating could skip no sector, so the later columns are loaded together, one round trip instead
+    // of one per stage.
+    *o += I + "bool all_alive = true;\n";
+    *o += I + "#pragma unroll\n";
+    *o += I + "for (int k = 0; k < " + sR + "; ++k) all_alive = all_alive && alive[k];\n";
+    *o += I + "if (__all_sync(GDV_FULL, all_alive)) {\n";
+    for (int st = 1; st < plan.stages(); ++st) stage(st, st == 1, true, I + "  ");
+    *o += I + "} else {\n";
+    for (int st = 1; st < plan.stages(); ++st) stage(st, true, false, I + "  ");
+    *o += I + "}\n";
+  } else {
+    for (int st = 1; st < plan.stages(); ++st) stage(st, true, false, I);
+  }
+  *o += I + "#pragma unroll\n";
+  *o += I + "for (int k = 0; k < " + sR + "; ++k) {\n";
+  *o += row;
+  *o += step_tail;
+  *o += I + "}\n";
+}
+
 void ReplaceAll(std::string* s, const std::string& from, const std::string& to) {
   for (size_t pos = 0; (pos = s->find(from, pos)) != std::string::npos; pos += to.size())
     s->replace(pos, from.size(), to);
@@ -2356,6 +2452,81 @@ void MarkHoisted(const BodyGen& gen, const Node& cond, std::vector<ColumnSlot>* 
   for (auto& sl : *slots)  // a dictionary / view row's validity also depends on its entry / view: read per row
     if (!sl.type.is_dict() && !sl.type.is_view() && std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end())
       sl.hoist = true;
+}
+
+void CollectFields(const Schema& schema, const Node& node, std::vector<int>* cols) {
+  switch (node.kind()) {
+    case NodeKind::kField: cols->push_back(schema.index_of(static_cast<const FieldNode&>(node).name())); return;
+    case NodeKind::kLiteral: return;
+    case NodeKind::kFunction:
+      for (const auto& c : static_cast<const FunctionNode&>(node).children()) CollectFields(schema, *c, cols);
+      return;
+    case NodeKind::kIf: {
+      const auto& n = static_cast<const IfNode&>(node);
+      CollectFields(schema, *n.condition(), cols);
+      CollectFields(schema, *n.then_node(), cols);
+      CollectFields(schema, *n.else_node(), cols);
+      return;
+    }
+    case NodeKind::kBoolean:
+      for (const auto& c : static_cast<const BooleanNode&>(node).children()) CollectFields(schema, *c, cols);
+      return;
+    case NodeKind::kIn: CollectFields(schema, *static_cast<const InNode&>(node).child(), cols); return;
+  }
+}
+
+void SpineConjuncts(const Node& node, std::vector<const Node*>* out) {
+  if (node.kind() == NodeKind::kBoolean && static_cast<const BooleanNode&>(node).op() == BooleanNode::kAnd) {
+    for (const auto& c : static_cast<const BooleanNode&>(node).children()) SpineConjuncts(*c, out);
+    return;
+  }
+  out->push_back(&node);
+}
+
+// Stage plan of a Filter condition over `slots`, or false when gating does not apply: some column
+// is not a plain fixed-width value (string, dictionary, view, bit-packed bool), the condition can
+// raise (errors must come from every row that holds the value), it has a single stage, or its first
+// stage reads more than half of the row's bytes.
+bool PlanGate(const Schema& schema, const Node& cond, const std::vector<ColumnSlot>& slots, GatePlan* plan) {
+  if (BodyGen::CanFail(cond)) return false;
+  for (const auto& sl : slots)
+    if (sl.type.is_varlen() || sl.type.is_bool()) return false;  // dictionaries and views are varlen
+  std::vector<const Node*> conj;
+  SpineConjuncts(cond, &conj);
+  // a conjunct waits for the last of its columns
+  std::vector<int> level(conj.size(), 0);
+  for (size_t c = 0; c < conj.size(); ++c) {
+    std::vector<int> cols;
+    CollectFields(schema, *conj[c], &cols);
+    for (int col : cols) {
+      int j = -1;
+      for (size_t s = 0; s < slots.size(); ++s)
+        if (slots[s].schema_index == col) j = static_cast<int>(s);
+      if (j < 0) return false;
+      level[c] = std::max(level[c], j);
+    }
+  }
+  std::vector<int> ends(level);
+  std::sort(ends.begin(), ends.end());
+  ends.erase(std::unique(ends.begin(), ends.end()), ends.end());
+  if (ends.size() < 2 || ends.back() != static_cast<int>(slots.size()) - 1) return false;
+  // The gated stages must carry most of the row: when stage 0 already reads more than half of the
+  // row's bytes, the most gating can save is less than the dependent round trip each later stage
+  // adds (`d * 100 < q AND date in range`: 16 of 20 B in stage 0, 7 % slower gated on an H100).
+  int row_bytes = 0, first_bytes = 0;
+  for (size_t s = 0; s < slots.size(); ++s) {
+    row_bytes += std::max(slots[s].type.width(), 1);
+    if (static_cast<int>(s) <= ends[0]) first_bytes += std::max(slots[s].type.width(), 1);
+  }
+  if (2 * first_bytes > row_bytes) return false;
+  plan->first_slot.assign(1, 0);
+  plan->conjuncts.assign(ends.size(), {});
+  for (size_t s = 0; s < ends.size(); ++s) {
+    plan->first_slot.push_back(ends[s] + 1);
+    for (size_t c = 0; c < conj.size(); ++c)
+      if (level[c] == ends[s]) plan->conjuncts[s].push_back(conj[c]);
+  }
+  return true;
 }
 
 int PickRowsPerThread(int in_bytes, int out_bytes, KernelKind kind) {
@@ -2864,6 +3035,22 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
   if (spec.kind == KernelKind::kFilter && spec.nullable && !gen.uses_ctx() && exprs.size() == 1)
     MarkHoisted(gen, *exprs[0]->root(), &slots);
+  // Fixed-width Filter: gated loads (EmitGatedGroup) wherever PlanGate finds a plan.  gate_seg[s] ANDs
+  // stage s's conjuncts into alive[k]; the segments come from a BodyGen of their own (over the same
+  // slots), whose globals replace those of `body`, which a gated kernel does not emit.
+  GatePlan gate;
+  std::vector<std::string> gate_seg;
+  std::vector<ColumnSlot> gate_slots = slots;
+  BodyGen sgen(schema, &gate_slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
+  if (spec.kind == KernelKind::kFilter && spec.filter_gating == 0 && exprs.size() == 1 &&
+      PlanGate(schema, *exprs[0]->root(), slots, &gate)) {
+    for (const auto& cj : gate.conjuncts) {
+      std::string seg, all;
+      for (const Node* c : cj) all += " && (" + sgen.GenTruth(*c, &seg, 6).v + ")";
+      gate_seg.push_back(seg + "            alive[k] = alive[k]" + all + ";\n");
+    }
+  }
+  const bool gated = !gate_seg.empty();
 
   int in_bytes = 0, out_bytes = 0;
   int n_varlen = 0;
@@ -2966,9 +3153,10 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   src += spec.nullable ? " (inputs may carry validity bitmaps)\n" : " (no input has nulls)\n";
   for (size_t i = 0; i < exprs.size(); ++i)
     src += "// expr_" + std::to_string(i) + ": " + CommentSafe(exprs[i]->ToString()) + "\n";
+  if (gated) src += "// gated loads: " + std::to_string(gate.stages()) + " stages\n";
   src += "#include \"gdv_device_lib.cuh\"\n";
   src += EmitArgsStruct(L);
-  src += gen.globals();
+  src += gated ? sgen.globals() : gen.globals();
   const std::string sR = std::to_string(R), sBT = std::to_string(BT);
   const std::string s32R = std::to_string(32 * R);
   // Fixed-width filters are bandwidth-bound and want every warp slot of the SM: ask for
@@ -2978,6 +3166,12 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
                !gen.uses_ctx() && body.size() < 6000;
   for (const auto& sl : slots)  // 128-bit math and string functions over dictionary views want registers
     light = light && !sl.type.is_decimal() && !sl.type.is_dict() && !sl.type.is_view();
+  if (light && W > 1 && gated) {
+    // the stage chain keeps more values live than the ungated group: hold the 48 warps per SM that
+    // the ungated kernel reaches at W > 1 (40 registers)
+    bounds += ", " + std::to_string(1536 / BT);
+    light = false;
+  }
   if (W > 1) light = false;  // W chunks keep 2 W more registers
   if (light) bounds += ", " + std::to_string(2048 / BT);
   src += "extern \"C\" __global__ void __launch_bounds__(" + bounds + ") " + spec.name +
@@ -2986,7 +3180,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   src += "  const u32 wid = threadIdx.x >> 5;\n";
   src += "  gdv_ctx ctx;\n  ctx.err = A.err;\n";
   EmitPrologue(slots, spec, &src);
-  src += gen.ScratchDecl(R);
+  src += gated ? sgen.ScratchDecl(R) : gen.ScratchDecl(R);
   if (stage_bytes > 0) {
     src += "  extern __shared__ uint4 gdv_smem[];\n";
     int vi = 0;
@@ -3197,9 +3391,17 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
       src += "        const i64 base = wbase + 32 * g;\n";
       src += "        if (base >= A.n) break;\n";
       src += "        if (base + " + s32R + " <= A.n) {\n";
-      EmitGroup(slots, spec, R, kFast, body, step_tail, &src, 5, 0, std::string(), coop);
+      const std::string gated_tail =
+          "          { const u32 m = __ballot_sync(GDV_FULL, in && alive[k]); if (lane == (u32)(g + k)) cur = m; }\n";
+      if (gated)
+        EmitGatedGroup(slots, spec, R, kFast, gate, gate_seg, gated_tail, &src, 5);
+      else
+        EmitGroup(slots, spec, R, kFast, body, step_tail, &src, 5, 0, std::string(), coop);
       src += "        } else {\n";
-      EmitGroup(slots, spec, R, kPred, body, step_tail, &src, 5, 0, std::string(), coop);
+      if (gated)
+        EmitGatedGroup(slots, spec, R, kPred, gate, gate_seg, gated_tail, &src, 5);
+      else
+        EmitGroup(slots, spec, R, kPred, body, step_tail, &src, 5, 0, std::string(), coop);
       src += "        }\n";
       src += "      }\n";
       src += "      mymask[w] = cur;\n";
@@ -3282,6 +3484,7 @@ Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>
   out->stages = staged ? S : 0;
   out->cta_tile_rows = static_cast<int64_t>(BT) * R;
   out->view_shortcuts = gen.view_shortcuts();
+  out->gated_stages = gated ? gate.stages() : 0;
   return Status::OK();
 }
 

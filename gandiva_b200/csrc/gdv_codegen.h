@@ -47,6 +47,7 @@ struct KernelSpec {
   int string_scan = 0;                // bit 0: LIKE with the per-lane matcher only (no cooperative scan);
                                       // bit 2: row-driven string filter even where the key-driven one applies
                                       // bit 3: no inline / prefix shortcut over string_view / binary_view views
+  int filter_gating = 0;              // fixed-width filter: 0 = gated loads wherever they apply, 1 = off
 };
 
 struct ColumnSlot {
@@ -79,6 +80,7 @@ struct GeneratedKernel {
   int stages = 0;                   // staged: shared-memory stages per CTA
   int64_t cta_tile_rows = 0;        // staged: rows per CTA tile (block_threads * rows_per_thread)
   int view_shortcuts = 0;           // call sites decided from the raw 16-byte views (BodyGen::ViewShortcut)
+  int gated_stages = 0;             // fixed-width filter: stages of gated loads (GatePlan), 0 = not gated
 };
 
 // Byte offsets inside gdv_args; the host packs the same layout (see EmitArgsStruct()).

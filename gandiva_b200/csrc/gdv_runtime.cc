@@ -320,6 +320,7 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
   spec.loader = cfg.loader;
   spec.stages = cfg.stages;
   spec.string_scan = cfg.string_scan;
+  spec.filter_gating = cfg.filter_gating;
   spec.large_batch = cfg.large_batch;
   const std::string placeholder = std::string(KernelPrefix(kind)) + "PLACEHOLDER";
   spec.name = placeholder;

@@ -130,6 +130,7 @@ struct Config {
   int stages = 0;
   int sm_reserve = 0;
   int string_scan = 0;
+  int filter_gating = 0;
   bool large_batch = false;  // set per kernel variant by Filter::KernelFor (batches >= 32 M rows)
 };
 

@@ -134,7 +134,10 @@ typedef struct gdv_config {
                               bit 3 (value 8): string_view / binary_view columns: no inline / prefix
                                      shortcut; equal, IN, starts_with and LIKE 'lit%...' read the row's
                                      bytes through the view like any other string function */
-  int32_t reserved[3];
+  int32_t filter_gating;   /* fixed-width Filter: 0 = engine decides (gated loads wherever they apply: a
+                              conjunct's columns are read only in rows the earlier conjuncts kept),
+                              1 = off (every column read for every row; the reference kernel) */
+  int32_t reserved[2];
 } gdv_config_t;
 void gdv_config_default(gdv_config_t* cfg);
 
@@ -309,7 +312,8 @@ gdv_status gdv_projector_kernel_info(gdv_projector_t p, char* name_buf, int64_t 
 /* Integer attribute of the kernel variant used by the latest Evaluate: "staged" (1 = TMA bulk
  * loader), "stages", "dynamic_smem", "cta_tile_rows", "tile_rows", "nullable",
  * "in_bytes_per_row", "view_shortcuts" (call sites decided from the 16-byte views of string_view /
- * binary_view columns: equal, IN, starts_with, LIKE 'lit%...'), "blocks_per_sm" (needs a device). */
+ * binary_view columns: equal, IN, starts_with, LIKE 'lit%...'), "gated_stages" (fixed-width Filter:
+ * stages of gated loads, 0 = not gated), "blocks_per_sm" (needs a device). */
 gdv_status gdv_projector_kernel_attr(gdv_projector_t p, const char* key, int64_t* out);
 void gdv_projector_release(gdv_projector_t p);
 
