@@ -772,28 +772,56 @@ class Projector:
 
     # -- device-resident path (bench / multi-GPU): raw pointers in HBM, caller-owned stream ----
     def evaluate_device(self, num_rows: int, columns: Sequence[tuple], outputs: Sequence[tuple],
-                        stream: int = 0, selection: tuple | None = None, sync: bool = False) -> None:
+                        stream: int = 0, selection: tuple | None = None, sync: bool = False) -> list | None:
         """columns: per schema field (validity_ptr|0, values_ptr, var_data_ptr|0, offset), where a
         dictionary-encoded column passes its indices as values and a gdv_dictionary_t as var_data, and
         a string_view / binary_view column its 16-byte views and a gdv_view_buffers_t (view_buffers());
-        outputs: per expression (validity_ptr|0, values_ptr); selection: (ptr, num_slots) or
-        (ptr, max_slots, d_count_ptr): the slot count is read from device memory (the d_count a
-        Filter.evaluate_device(..., sync=False) wrote on the same stream), no host round trip."""
+        outputs: per expression (validity_ptr|0, values_ptr), or for a utf8 / binary output
+        (validity_ptr|0, offsets_ptr, var_data_ptr, var_capacity) with room for num_slots + 1 int32
+        offsets; selection: (ptr, num_slots) or (ptr, max_slots, d_count_ptr): the slot count is read
+        from device memory (the d_count a Filter.evaluate_device(..., sync=False) wrote on the same
+        stream), no host round trip.  A utf8 / binary output whose bytes exceed its var_capacity raises
+        ExecutionError here (sync=True) or from sync().  With sync=True returns each output's var_size
+        (bytes written; None for fixed-width outputs)."""
+        cb, _keep = self._device_batch(num_rows, columns)
+        outs = (gdv_out_column_t * max(len(outputs), 1))()
+        for i, o in enumerate(outputs):
+            outs[i].validity, outs[i].values = (o[0] or None), (o[1] or None)
+            if len(o) > 2:
+                outs[i].var_data, outs[i].var_capacity = (o[2] or None), o[3]
+        s = self._device_selection(selection)
+        _check(lib.gdv_projector_evaluate(self._h, C.byref(cb), None if s is None else C.byref(s), outs, len(outputs),
+                                          _stream_handle(stream), 0 if sync else 1))
+        if sync:
+            return [outs[i].var_size if len(o) > 2 else None for i, o in enumerate(outputs)]
+        return None
+
+    def output_var_size_device(self, num_rows: int, columns: Sequence[tuple], index: int, stream: int = 0,
+                               selection: tuple | None = None) -> int:
+        """Exact var_data bytes of utf8 / binary output `index` over a device batch (columns and selection as
+        in evaluate_device; with a d_count_ptr the count is read on the device).  Runs the sizing pass and
+        the scan and synchronises the stream: one round trip, for callers who want an exact buffer rather
+        than an upper bound."""
+        cb, _keep = self._device_batch(num_rows, columns)
+        s = self._device_selection(selection)
+        need = C.c_int64(0)
+        _check(lib.gdv_projector_output_var_size(self._h, C.byref(cb), None if s is None else C.byref(s), index,
+                                                 _stream_handle(stream), C.byref(need)))
+        return need.value
+
+    @staticmethod
+    def _device_batch(num_rows: int, columns: Sequence[tuple]):
         cols = (gdv_column_t * max(len(columns), 1))()
         for i, (vld, val, var, off) in enumerate(columns):
             cols[i].validity, cols[i].values, cols[i].var_data, cols[i].offset = \
                 (vld or None), (val or None), _var_ptr(var), off
-        cb = gdv_batch_t(num_rows, len(columns), GDV_MEM_DEVICE, cols)
-        outs = (gdv_out_column_t * max(len(outputs), 1))()
-        for i, (vld, val) in enumerate(outputs):
-            outs[i].validity, outs[i].values = (vld or None), (val or None)
-        csel = None
-        if selection is not None:
-            s = gdv_selection_t(selection[0], selection[1], selection[1], self._mode, GDV_MEM_DEVICE, 0,
-                                selection[2] if len(selection) > 2 else None)
-            csel = C.byref(s)
-        _check(lib.gdv_projector_evaluate(self._h, C.byref(cb), csel, outs, len(outputs),
-                                          _stream_handle(stream), 0 if sync else 1))
+        return gdv_batch_t(num_rows, len(columns), GDV_MEM_DEVICE, cols), cols
+
+    def _device_selection(self, selection: tuple | None):
+        if selection is None:
+            return None
+        return gdv_selection_t(selection[0], selection[1], selection[1], self._mode, GDV_MEM_DEVICE, 0,
+                               selection[2] if len(selection) > 2 else None)
 
     def sync(self, stream: int = 0) -> None:
         _check(lib.gdv_projector_sync(self._h, _stream_handle(stream)))

@@ -86,12 +86,20 @@ extern "C" __global__ void __launch_bounds__(256) gdv_fill_u32(u32* p, i64 words
 // ---- string-producing projections: exclusive scan of the per-tile byte counts -------------------
 // One CTA of 1024 threads walks the tile array in blocks of 1024 (a 1e9-row batch has ~2M tiles of
 // 512 rows: a few hundred microseconds next to the two passes over the string bytes).  Writes the
-// total to *total and raises GDV_ERR_OFFSET_OVERFLOW when it exceeds `limit` (int32 offsets).
+// total to *total; above `limit` it raises GDV_ERR_OFFSET_OVERFLOW when the total does not fit int32
+// offsets, else GDV_ERR_VAR_CAPACITY (`limit` is then the caller's var_data capacity).
+// With `n_ptr` (a slot count in device memory, gdv_selection_t.d_num_slots) only the tiles that hold
+// its first min(*n_ptr, n_tiles * tile_rows) rows are scanned: the sizing pass wrote no others, and a
+// selective Filter leaves far fewer tiles than the host-side bound this one CTA would otherwise walk.
 extern "C" __global__ void __launch_bounds__(1024)
-gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit) {
+gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit, const u64* n_ptr, i64 tile_rows) {
   __shared__ u64 s_warp[32];
   __shared__ u64 s_carry;
   const u32 lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+  if (n_ptr != nullptr) {
+    const u64 c = *n_ptr;
+    if (c < (u64)n_tiles * (u64)tile_rows) n_tiles = (i64)((c + (u64)tile_rows - 1ull) / (u64)tile_rows);
+  }
   if (threadIdx.x == 0) s_carry = 0ull;
   __syncthreads();
   for (i64 b = 0; b < n_tiles; b += 1024) {
@@ -122,7 +130,8 @@ gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit) {
   }
   if (threadIdx.x == 0) {
     *total = s_carry;
-    if (s_carry > limit && err != nullptr) atomicCAS(err, 0, GDV_ERR_OFFSET_OVERFLOW);
+    if (s_carry > limit && err != nullptr)
+      atomicCAS(err, 0, s_carry > 0x7fffffffull ? GDV_ERR_OFFSET_OVERFLOW : GDV_ERR_VAR_CAPACITY);
   }
 }
 

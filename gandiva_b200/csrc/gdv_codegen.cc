@@ -2626,6 +2626,8 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
     }
   }
   src += "  __shared__ u64 s_part[" + std::to_string(NW) + "];\n";
+  if (has_sel && !is_size)  // a device count of 0 leaves no tile to write offsets[0]
+    src += "  if (A.n == 0 && blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<i32*>(A.out_val[0])[0] = 0;\n";
   src += "  const i64 n_tiles = (A.n + " + std::to_string(T - 1) + ") / " + sT + ";\n";
   src += "  for (i64 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {\n";
   src += "    const i64 base = tile * " + sT + " + (i64)wid * " + s32R + ";\n";
@@ -2738,6 +2740,9 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   }
   src += "  }\n";
   src += "}\n";
+  // selection-vector projectors may read the slot count from device memory: both passes then cover
+  // the device count's tiles and rows only (the scan stops at the same tile, gdv_scan_tiles)
+  if (has_sel) ApplyDeviceCount(&src);
 
   out->source = std::move(src);
   out->name = spec.name;

@@ -974,6 +974,18 @@ Status Projector::CheckEvaluateArgs(const gdv_batch_t* batch, const gdv_selectio
   return Status::OK();
 }
 
+// The two-stage rope plan sizes its temporaries on the host, synchronously, so it cannot take part in
+// a chain that keeps the slot count on the device: its utf8/binary outputs refuse d_num_slots.  (Its
+// fixed-width outputs have always accepted it, and still do.)  Host batches fall through to the
+// "d_num_slots needs device buffers" of the evaluation itself.
+Status Projector::RefuseDeviceCountWithRopeTemps(const gdv_batch_t* batch, const gdv_selection_t* sel) const {
+  if (sel == nullptr || sel->mode == GDV_SEL_NONE || sel->d_num_slots == nullptr || batch->mem_space == GDV_MEM_HOST)
+    return Status::OK();
+  return Status::Make(GDV_NOT_IMPLEMENTED,
+                      "d_num_slots: a utf8/binary output of a projector that materialises rope temporaries (the "
+                      "two-stage rope plan) needs the slot count on the host; its temporaries are sized there");
+}
+
 Status Projector::OutputVarSize(const gdv_batch_t* batch, const gdv_selection_t* sel, int out_index,
                                 void* stream, int64_t* bytes) {
   if (bytes == nullptr) return Status::Make(GDV_INVALID, "null argument");
@@ -982,6 +994,8 @@ Status Projector::OutputVarSize(const gdv_batch_t* batch, const gdv_selection_t*
     return Status::Make(GDV_INVALID, "output index out of range");
   if (rope_main_ != nullptr) {
     if (batch == nullptr) return Status::Make(GDV_INVALID, "null argument");
+    for (const auto& sk : rope_main_->strings_)
+      if (sk.out_index == out_index) GDV_RETURN_NOT_OK(RefuseDeviceCountWithRopeTemps(batch, sel));
     TempColumns tc;
     GDV_RETURN_NOT_OK(tc.Build(rope_pre_.get(), batch, stream));
     return rope_main_->OutputVarSize(&tc.batch, sel, out_index, stream, bytes);  // synchronous: reads the total back
@@ -999,9 +1013,12 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
                                  bool async, bool size_only, int64_t* total_out) {
   int64_t n = 0;
   GDV_RETURN_NOT_OK(CheckEvaluateArgs(batch, sel, &n));
-  if (sel != nullptr && sel->d_num_slots != nullptr)
-    return Status::Make(GDV_NOT_IMPLEMENTED, "utf8/binary outputs need the slot count on the host (d_num_slots is for fixed-width outputs)");
   const bool host = batch->mem_space == GDV_MEM_HOST;
+  // Device slot count: n is only the upper bound the grids and the tile array are sized with; both
+  // passes and the scan read the count on the device, and the scan checks the total against the
+  // caller's var_capacity (the host never sees the total before the write pass).
+  const bool dev_count = selection_mode_ != GDV_SEL_NONE && sel->d_num_slots != nullptr;
+  if (dev_count && host) return Status::Make(GDV_INVALID, "d_num_slots needs device buffers");
   Device* dev = nullptr;
   GDV_RETURN_NOT_OK(Device::Get(cfg_.device, &dev));
   CompiledKernel *ksize = nullptr, *kwrite = nullptr;
@@ -1031,6 +1048,11 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
         GDV_RETURN_NOT_OK(StagedHtoD(dev, dsel, sel->indices, bytes, stream));
     }
     Put<CUdeviceptr>(args, L.off_sel, dsel);
+    if (dev_count) Put<CUdeviceptr>(args, L.off_n_ptr, reinterpret_cast<CUdeviceptr>(sel->d_num_slots));
+  }
+  if (dev_count && !size_only) {
+    if (out == nullptr || out->values == nullptr) return Status::Make(GDV_INVALID, "output offsets buffer is null");
+    if (out->var_capacity < 0) return Status::Make(GDV_INVALID, "negative var_capacity");
   }
   // [total u64][pad u64][one u64 per CTA tile]; lives until the stream is synchronised
   const int64_t T = gen.tile_rows;
@@ -1048,6 +1070,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
       GDV_RETURN_NOT_OK(CuCheck(d.MemsetD8Async(pend.d_err, 0, 256, stream), "memset err"));
     }
     d_err = pend.d_err;
+    if (dev_count && !size_only) pend.var_checks.push_back({d_state, out->var_capacity, sk->out_index});
   }
   Put<CUdeviceptr>(args, L.off_err, d_err);
   Put<CUdeviceptr>(args, L.off_tile_state, d_state + 16);
@@ -1060,9 +1083,11 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
     CUfunction scan = nullptr;
     GDV_RETURN_NOT_OK(dev->StaticFunction("gdv_scan_tiles", &scan));
     CUdeviceptr tiles = d_state + 16, total = d_state, errp = d_err;
-    int64_t nt = n_tiles;
+    CUdeviceptr n_ptr = dev_count ? reinterpret_cast<CUdeviceptr>(sel->d_num_slots) : 0;
+    int64_t nt = n_tiles, tile_rows = T;
     uint64_t limit = 0x7fffffffull;
-    void* params[] = {&tiles, &nt, &total, &errp, &limit};
+    if (dev_count && !size_only) limit = std::min<uint64_t>(limit, static_cast<uint64_t>(out->var_capacity));
+    void* params[] = {&tiles, &nt, &total, &errp, &limit, &n_ptr, &tile_rows};
     g_launch_count.fetch_add(1);
     GDV_RETURN_NOT_OK(CuCheck(d.LaunchKernel(scan, 1, 1, 1, 1024, 1, 1, 0, stream, params, nullptr),
                               "cuLaunchKernel(gdv_scan_tiles)"));
@@ -1131,6 +1156,7 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
   if (rope_main_ != nullptr) {
     if (batch->num_columns != static_cast<int>(schema_->fields().size()))
       return Status::Make(GDV_INVALID, "RecordBatch schema must match the schema of Make()");
+    if (!rope_main_->strings_.empty()) GDV_RETURN_NOT_OK(RefuseDeviceCountWithRopeTemps(batch, sel));
     TempColumns tc;
     GDV_RETURN_NOT_OK(tc.Build(rope_pre_.get(), batch, stream_v));
     Status st = rope_main_->Evaluate(&tc.batch, sel, all_outs, n_all_outs, stream_v, async);
@@ -1284,13 +1310,25 @@ Status Projector::Sync(void* stream_v) {
   Status copy = Status::OK();
   if (have && pend.d_err != 0) copy = CuCheck(d.MemcpyDtoHAsync(&err, pend.d_err, sizeof(int), stream), "D2H err");
   Status s = CuCheck(d.StreamSynchronize(stream), "cuStreamSynchronize");
+  std::string detail;  // a capacity error of a device-count string output: which output, how many bytes
+  if (copy.ok() && s.ok() && err == 3) {
+    for (const auto& vc : pend.var_checks) {
+      uint64_t total = 0;
+      if (d.MemcpyDtoHAsync(&total, vc.d_total, 8, stream) != CUDA_SUCCESS || d.StreamSynchronize(stream) != CUDA_SUCCESS) break;
+      if (total > static_cast<uint64_t>(vc.capacity)) {
+        detail = ": output " + std::to_string(vc.out_index) + " needs " + std::to_string(total) +
+                 " bytes, its var_capacity is " + std::to_string(vc.capacity);
+        break;
+      }
+    }
+  }
   if (have) {  // on every path: the pending blocks go back to the pool once the stream is idle
     if (pend.d_err != 0) dev->Free(pend.d_err);
     for (auto p : pend.scratch) dev->Free(p);
   }
   GDV_RETURN_NOT_OK(copy);
   GDV_RETURN_NOT_OK(s);
-  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, ExecutionErrorMessage(err));
+  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, ExecutionErrorMessage(err) + detail);
   return Status::OK();
 }
 

@@ -167,6 +167,14 @@ struct Pending {
   CUdeviceptr d_bits = 0;   // dictionary-first filter: one bit per dictionary entry
   size_t bits_cap = 0;
   bool uses_ctx = false;
+  // projector, utf8/binary outputs with a device slot count: where each scan left its byte total,
+  // the output's var_capacity and index (they name the output a capacity error is about)
+  struct VarCheck {
+    CUdeviceptr d_total;
+    int64_t capacity;
+    int out_index;
+  };
+  std::vector<VarCheck> var_checks;
 };
 
 class Projector {
@@ -175,7 +183,8 @@ class Projector {
                      const Config& cfg, std::shared_ptr<Projector>* out);
   Status Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel, gdv_out_column_t* outs,
                   int n_outs, void* stream, bool async);
-  // Bytes output `out_index` (utf8/binary) produces for this batch: runs the sizing pass only.
+  // Bytes output `out_index` (utf8/binary) produces for this batch: runs the sizing pass and the scan,
+  // over sel->d_num_slots when given (then synchronises to read the total back).
   Status OutputVarSize(const gdv_batch_t* batch, const gdv_selection_t* sel, int out_index,
                        void* stream, int64_t* bytes);
   Status Sync(void* stream);
@@ -205,6 +214,7 @@ class Projector {
   Status StringKernelsFor(StringKernels* sk, bool nullable, CompiledKernel** size,
                           CompiledKernel** write);
   Status CheckEvaluateArgs(const gdv_batch_t* batch, const gdv_selection_t* sel, int64_t* n) const;
+  Status RefuseDeviceCountWithRopeTemps(const gdv_batch_t* batch, const gdv_selection_t* sel) const;
   Status EvaluateString(StringKernels* sk, const gdv_batch_t* batch, const gdv_selection_t* sel,
                         gdv_out_column_t* out, void* stream, bool async, bool size_only,
                         int64_t* total);

@@ -239,8 +239,19 @@ typedef struct gdv_selection {
   const void* d_num_slots; /* projector, device buffers, may be NULL: device uint64 holding the slot
                          count (e.g. the d_count a Filter wrote on the same stream).  The kernel reads
                          it on the device, so a Filter -> Projector chain needs no host round trip;
-                         num_slots is then only an upper bound (grid size, output capacity).  Rows past
-                         the device count are not written.  Fixed-width outputs only. */
+                         num_slots is then only an upper bound (grid size, output capacity): the kernels
+                         use c = min(*d_num_slots, num_slots) rows.  Rows past c are not written: no
+                         value, no offset past offsets[c], no byte past offsets[c], no validity word that
+                         lies wholly past c (in the word holding row c-1 the bits past it are 0).
+                         utf8/binary outputs: values holds num_slots + 1 int32 offsets and var_data
+                         var_capacity bytes, an upper bound the caller picks; the byte total is
+                         offsets[c].  var_size is the total after a synchronous call, -1 after an async
+                         one.  A total above var_capacity is an ExecutionError (from the call when it is
+                         synchronous, else from gdv_projector_sync) and no byte past var_capacity is
+                         stored.  gdv_projector_output_var_size over a d_num_slots selection returns the
+                         exact total (one round trip).  Device buffers only (GDV_INVALID otherwise);
+                         utf8/binary outputs of a projector that materialises rope temporaries (the
+                         two-stage rope plan) refuse it with GDV_NOT_IMPLEMENTED. */
 } gdv_selection_t;
 
 /* ---- library / device ---------------------------------------------------- */
@@ -300,7 +311,10 @@ gdv_status gdv_projector_evaluate(gdv_projector_t p, const gdv_batch_t* batch,
                                   int32_t n_outs, void* stream, int32_t async);
 gdv_status gdv_projector_sync(gdv_projector_t p, void* stream);
 /* Bytes needed for output i's var_data given the batch (utf8/binary outputs): runs the
- * sizing pass only.  Fixed-width outputs return 0. */
+ * sizing pass and the scan, then synchronises the stream.  Fixed-width outputs return 0.  With
+ * selection->d_num_slots it sizes the rows of the device count: the opt-in path for a caller of a
+ * device-resident Filter -> Projector chain who wants an exact buffer rather than an upper bound,
+ * at the cost of one host round trip. */
 gdv_status gdv_projector_output_var_size(gdv_projector_t p, const gdv_batch_t* batch,
                                          const gdv_selection_t* selection, int32_t out_index,
                                          void* stream, int64_t* out_bytes);
