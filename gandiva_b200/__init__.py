@@ -23,7 +23,7 @@ import pyarrow as pa
 
 __all__ = [
     "TreeExprBuilder", "Node", "Expression", "Condition", "Configuration", "SelectionVector",
-    "Projector", "Filter", "FunctionSignature", "make_projector", "make_filter",
+    "Projector", "Filter", "FunctionSignature", "FunctionRegistry", "make_projector", "make_filter",
     "get_registered_function_signatures", "GandivaError", "cuda_available", "lib",
 ]
 
@@ -66,7 +66,13 @@ class gdv_config_t(C.Structure):
     _fields_ = [("optimize", C.c_int32), ("dump_ir", C.c_int32), ("device", C.c_int32),
                 ("rows_per_thread", C.c_int32), ("block_threads", C.c_int32),
                 ("loader", C.c_int32), ("sm_reserve", C.c_int32), ("stages", C.c_int32),
-                ("string_scan", C.c_int32), ("filter_gating", C.c_int32), ("reserved", C.c_int32 * 2)]
+                ("string_scan", C.c_int32), ("filter_gating", C.c_int32), ("function_registry", C.c_void_p)]
+
+
+class gdv_function_def_t(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("params", C.POINTER(gdv_type_t)), ("n_params", C.c_int32),
+                ("ret", gdv_type_t), ("null_mode", C.c_int32), ("can_raise", C.c_int32),
+                ("body", C.c_char_p), ("prelude", C.c_char_p)]
 
 
 class gdv_column_t(C.Structure):
@@ -167,6 +173,11 @@ def _load() -> C.CDLL:
         "gdv_filter_release": (None, [vp]),
         "gdv_registry_size": (i32, []),
         "gdv_registry_get": (i32, [i32, P(C.c_char_p), P(gdv_type_t), P(gdv_type_t), i32, P(i32)]),
+        "gdv_function_registry_create": (i32, [P(vp)]),
+        "gdv_function_registry_release": (None, [vp]),
+        "gdv_function_registry_add": (i32, [vp, P(gdv_function_def_t)]),
+        "gdv_function_registry_signatures": (i32, [vp]),
+        "gdv_function_registry_get": (i32, [vp, i32, P(C.c_char_p), P(gdv_type_t), P(gdv_type_t), i32, P(i32)]),
         "gdv_host_alloc": (i32, [C.c_size_t, P(vp)]),
         "gdv_host_free": (i32, [vp]),
         "gdv_generate_lineitem": (i32, [i32, i32, C.c_uint64, i64, i64, vp, vp, i32, vp]),
@@ -512,7 +523,9 @@ class Configuration:
 
     def __init__(self, optimize: bool = True, dump_ir: bool = False, device: int = 0,
                  rows_per_thread: int = 0, block_threads: int = 0, loader: int = 0,
-                 sm_reserve: int = 0, stages: int = 0, string_scan: int = 0, filter_gating: int = 0):
+                 sm_reserve: int = 0, stages: int = 0, string_scan: int = 0, filter_gating: int = 0,
+                 function_registry: "FunctionRegistry | None" = None):
+        self.function_registry = function_registry
         self.stages = int(stages)
         self.string_scan = int(string_scan)
         self.filter_gating = int(filter_gating)
@@ -537,6 +550,8 @@ class Configuration:
         c.stages = self.stages
         c.string_scan = self.string_scan
         c.filter_gating = self.filter_gating
+        if self.function_registry is not None:
+            c.function_registry = self.function_registry._h
         return c
 
 
@@ -1091,6 +1106,51 @@ class FunctionSignature:
 
     def __str__(self) -> str:
         return "%s %s(%s)" % (self._ret, self._name, ", ".join(str(p) for p in self._params))
+
+
+_NULL_MODES = {"if_null": 0, "never": 1, "internal": 2}
+
+
+class FunctionRegistry:
+    """Functions the caller adds to the engine as CUDA text (include/gandiva_b200.h, "user-defined
+    functions", has the calling convention).  `Configuration(function_registry=reg)` makes a Projector or
+    Filter resolve names against the built-ins first and `reg` second; the fuser writes each user function
+    a kernel calls into that kernel.  Functions can be registered until the registry is first used by
+    make_projector / make_filter."""
+
+    def __init__(self):
+        h = C.c_void_p()
+        _check(lib.gdv_function_registry_create(C.byref(h)))
+        self._h = h.value
+
+    def __del__(self):
+        if getattr(self, "_h", None) and lib is not None:
+            lib.gdv_function_registry_release(self._h)
+            self._h = None
+
+    def register(self, name: str, param_types: list, return_type: pa.DataType, body: str, *,
+                 null_mode: str = "if_null", can_raise: bool = False, prelude: str = "") -> None:
+        """`body`: the statements of the device function; parameters are a0, a1, ... (plus v0, v1, ... with
+        null_mode "never" / "internal", `out_valid` with "internal", `ctx` with can_raise)."""
+        if null_mode not in _NULL_MODES:
+            raise ValueError("null_mode must be one of %s, not %r" % (sorted(_NULL_MODES), null_mode))
+        params = (gdv_type_t * max(1, len(param_types)))(*[_to_c_type(t) for t in param_types])
+        d = gdv_function_def_t(name.encode(), params, len(param_types), _to_c_type(return_type),
+                               _NULL_MODES[null_mode], int(bool(can_raise)), body.encode(), prelude.encode())
+        _check(lib.gdv_function_registry_add(self._h, C.byref(d)))
+
+    def signatures(self) -> list:
+        """The signatures of this registry only (get_registered_function_signatures() lists the built-ins)."""
+        out = []
+        for i in range(lib.gdv_function_registry_signatures(self._h)):
+            name = C.c_char_p()
+            ret = gdv_type_t()
+            params = (gdv_type_t * 16)()
+            n = C.c_int32()
+            _check(lib.gdv_function_registry_get(self._h, i, C.byref(name), C.byref(ret), params, 16, C.byref(n)))
+            out.append(FunctionSignature(name.value.decode(), _from_c_type(ret),
+                                         [_from_c_type(params[k]) for k in range(min(n.value, 16))]))
+        return out
 
 
 def generate_lineitem(device: int, kind: int, seed: int, first_row: int, num_rows: int,

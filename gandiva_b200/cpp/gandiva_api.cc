@@ -14,6 +14,7 @@
 #include "gandiva/expression.h"
 #include "gandiva/expression_registry.h"
 #include "gandiva/filter.h"
+#include "gandiva/function_registry.h"
 #include "gandiva/function_signature.h"
 #include "gandiva/node.h"
 #include "gandiva/projector.h"
@@ -173,6 +174,8 @@ gdv_config_t ConfigToC(const std::shared_ptr<Configuration>& c) {
     cfg.optimize = c->optimize() ? 1 : 0;
     cfg.dump_ir = c->dump_ir() ? 1 : 0;
     cfg.device = c->device();
+    if (c->function_registry() != nullptr)
+      cfg.function_registry = static_cast<gdv_function_registry_t>(c->function_registry()->handle());
   }
   return cfg;
 }
@@ -728,6 +731,53 @@ std::vector<std::shared_ptr<FunctionSignature>> GetRegisteredFunctionSignatures(
     DataTypeVector pts;
     for (int32_t k = 0; k < np && k < 16; ++k) pts.push_back(FromC(params[k]));
     out.push_back(std::make_shared<FunctionSignature>(name, std::move(pts), FromC(ret)));
+  }
+  return out;
+}
+
+// ---- user-defined functions ----------------------------------------------------------------------
+FunctionRegistry::FunctionRegistry() {
+  gdv_function_registry_t h = nullptr;
+  gdv_function_registry_create(&h);
+  handle_ = h;
+}
+
+FunctionRegistry::~FunctionRegistry() { gdv_function_registry_release(static_cast<gdv_function_registry_t>(handle_)); }
+
+Status FunctionRegistry::Register(const FunctionSignature& signature, const std::string& body, NullMode null_mode,
+                                  bool can_raise, const std::string& prelude) {
+  std::vector<gdv_type_t> params;
+  for (const auto& t : signature.param_types()) {
+    if (t == nullptr) return Status::Invalid("parameter type cannot be null");
+    params.push_back(ToC(*t));
+  }
+  if (signature.ret_type() == nullptr) return Status::Invalid("return type cannot be null");
+  gdv_function_def_t def;
+  std::memset(&def, 0, sizeof(def));
+  def.name = signature.base_name().c_str();
+  def.params = params.data();
+  def.n_params = static_cast<int32_t>(params.size());
+  def.ret = ToC(*signature.ret_type());
+  def.null_mode = static_cast<int32_t>(null_mode);
+  def.can_raise = can_raise ? 1 : 0;
+  def.body = body.c_str();
+  def.prelude = prelude.c_str();
+  return ToStatus(gdv_function_registry_add(static_cast<gdv_function_registry_t>(handle_), &def));
+}
+
+std::vector<FunctionSignature> FunctionRegistry::GetSignatures() const {
+  std::vector<FunctionSignature> out;
+  auto reg = static_cast<gdv_function_registry_t>(handle_);
+  const int32_t n = gdv_function_registry_signatures(reg);
+  for (int32_t i = 0; i < n; ++i) {
+    const char* name = nullptr;
+    gdv_type_t ret;
+    gdv_type_t params[16];
+    int32_t np = 0;
+    if (gdv_function_registry_get(reg, i, &name, &ret, params, 16, &np) != GDV_OK) continue;
+    DataTypeVector pts;
+    for (int32_t k = 0; k < np && k < 16; ++k) pts.push_back(FromC(params[k]));
+    out.emplace_back(name, std::move(pts), FromC(ret));
   }
   return out;
 }

@@ -34,6 +34,20 @@ namespace {
 
 NodeH* N(gdv_node_t h) { return reinterpret_cast<NodeH*>(h); }
 
+struct FunctionRegistryH {
+  std::shared_ptr<FunctionRegistry> p;
+};
+
+gdv_status GetSignature(const FunctionDef& d, const char** name, gdv_type_t* ret, gdv_type_t* params,
+                        int32_t max_params, int32_t* n_params) {
+  if (name) *name = d.name.c_str();
+  if (ret) *ret = d.ret.c();
+  if (n_params) *n_params = static_cast<int32_t>(d.params.size());
+  for (int32_t k = 0; params != nullptr && k < max_params && k < static_cast<int32_t>(d.params.size()); ++k)
+    params[k] = d.params[k].c();
+  return GDV_OK;
+}
+
 int64_t CopyOut(const std::string& s, char* buf, int64_t len) {
   if (buf != nullptr && len > 0) {
     const size_t n = std::min(static_cast<size_t>(len - 1), s.size());
@@ -56,6 +70,11 @@ Config FromC(const gdv_config_t* c) {
     cfg.string_scan = c->string_scan;
     cfg.filter_gating = c->filter_gating;
     cfg.sm_reserve = c->sm_reserve;
+    if (c->function_registry != nullptr) {
+      const auto& reg = reinterpret_cast<FunctionRegistryH*>(c->function_registry)->p;
+      reg->Freeze();
+      cfg.functions = reg;
+    }
   }
   return cfg;
 }
@@ -414,13 +433,48 @@ gdv_status gdv_registry_get(int32_t i, const char** name, gdv_type_t* ret, gdv_t
                             int32_t max_params, int32_t* n_params) {
   const auto& all = Registry::Get().all();
   if (i < 0 || i >= static_cast<int32_t>(all.size())) return Fail(GDV_INVALID, "index out of range");
-  const FunctionDef& d = all[i];
-  if (name) *name = d.name.c_str();
-  if (ret) *ret = d.ret.c();
-  if (n_params) *n_params = static_cast<int32_t>(d.params.size());
-  for (int32_t k = 0; params != nullptr && k < max_params && k < static_cast<int32_t>(d.params.size()); ++k)
-    params[k] = d.params[k].c();
+  return GetSignature(all[i], name, ret, params, max_params, n_params);
+}
+
+// ---- user-defined functions ------------------------------------------------------------------
+gdv_status gdv_function_registry_create(gdv_function_registry_t* out) {
+  if (out == nullptr) return Fail(GDV_INVALID, "null argument");
+  *out = reinterpret_cast<gdv_function_registry_t>(new FunctionRegistryH{std::make_shared<FunctionRegistry>()});
   return GDV_OK;
+}
+
+void gdv_function_registry_release(gdv_function_registry_t reg) { delete reinterpret_cast<FunctionRegistryH*>(reg); }
+
+gdv_status gdv_function_registry_add(gdv_function_registry_t reg, const gdv_function_def_t* def) {
+  if (reg == nullptr || def == nullptr || def->name == nullptr || def->body == nullptr ||
+      (def->n_params > 0 && def->params == nullptr) || def->n_params < 0)
+    return Fail(GDV_INVALID, "null argument");
+  if (def->null_mode < GDV_NULL_IF_NULL || def->null_mode > GDV_NULL_INTERNAL)
+    return Fail(GDV_INVALID, "null_mode must be GDV_NULL_IF_NULL, GDV_NULL_NEVER or GDV_NULL_INTERNAL");
+  UserFunction fn;
+  fn.name = def->name;
+  for (int32_t i = 0; i < def->n_params; ++i) fn.params.push_back(DataType(def->params[i]));
+  fn.ret = DataType(def->ret);
+  fn.nulls = def->null_mode == GDV_NULL_NEVER ? NullMode::kNever
+             : def->null_mode == GDV_NULL_INTERNAL ? NullMode::kInternal : NullMode::kIfNull;
+  fn.can_raise = def->can_raise != 0;
+  fn.body = def->body;
+  if (def->prelude != nullptr) fn.prelude = def->prelude;
+  Status s = reinterpret_cast<FunctionRegistryH*>(reg)->p->Register(fn);
+  return s.ok() ? GDV_OK : Fail(s);
+}
+
+int32_t gdv_function_registry_signatures(gdv_function_registry_t reg) {
+  if (reg == nullptr) return 0;
+  return static_cast<int32_t>(reinterpret_cast<FunctionRegistryH*>(reg)->p->all().size());
+}
+
+gdv_status gdv_function_registry_get(gdv_function_registry_t reg, int32_t i, const char** name, gdv_type_t* ret,
+                                     gdv_type_t* params, int32_t max_params, int32_t* n_params) {
+  if (reg == nullptr) return Fail(GDV_INVALID, "null registry");
+  const auto& all = reinterpret_cast<FunctionRegistryH*>(reg)->p->all();
+  if (i < 0 || i >= static_cast<int32_t>(all.size())) return Fail(GDV_INVALID, "index out of range");
+  return GetSignature(all[static_cast<size_t>(i)], name, ret, params, max_params, n_params);
 }
 
 // ---- harness helpers ----------------------------------------------------------------------

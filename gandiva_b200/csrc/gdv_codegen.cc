@@ -100,7 +100,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
         if (!s.ok()) return s;
         params.push_back(c->return_type());
       }
-      const FunctionDef* def = Registry::Get().Lookup(fn.name(), params);
+      const FunctionDef* def = LookupFunction(fn.name(), params);
       if (def == nullptr) {
         std::string sig = fn.return_type().ToString() + " " + fn.name() + "(";
         for (size_t i = 0; i < params.size(); ++i)
@@ -537,7 +537,7 @@ class BodyGen {
         const auto& fn = static_cast<const FunctionNode&>(node);
         std::vector<DataType> params;
         for (const auto& c : fn.children()) params.push_back(c->return_type());
-        const FunctionDef* def = Registry::Get().Lookup(fn.name(), params);
+        const FunctionDef* def = LookupFunction(fn.name(), params);
         if (def == nullptr || def->nulls != NullMode::kIfNull || (def->flags & (kConcat | kVirtual)) || fn.name() == "nvl")
           return;
         for (const auto& c : fn.children()) ValueStrict(*c, cols);
@@ -578,7 +578,7 @@ class BodyGen {
         const auto& fn = static_cast<const FunctionNode&>(node);
         std::vector<DataType> params;
         for (const auto& c : fn.children()) params.push_back(c->return_type());
-        const FunctionDef* def = Registry::Get().Lookup(fn.name(), params);
+        const FunctionDef* def = LookupFunction(fn.name(), params);
         if (def != nullptr && (def->flags & kCanFail)) return true;
         if (ArgGuard(fn) >= 0) return true;
         for (const auto& c : fn.children())
@@ -949,13 +949,27 @@ class BodyGen {
     return name;
   }
 
+  // A user function's prelude and definition go into the kernel's file scope at its first call site, each once
+  // (two functions of one registry may share a prelude).
+  void EmitUserFunction(const FunctionDef& def) {
+    auto once = [&](const std::string& text) {
+      if (text.empty() || std::find(user_text_.begin(), user_text_.end(), text) != user_text_.end()) return;
+      user_text_.push_back(text);
+      globals_ += text;
+    };
+    if (def.flags & kCanFail) once(kUserRaiseHelper);
+    once(def.prelude);
+    once(def.source);
+  }
+
   Val GenFunction(const FunctionNode& fn, std::string* out, int indent) {
     std::vector<DataType> ptypes;
     for (const auto& c : fn.children()) ptypes.push_back(c->return_type());
-    const FunctionDef* def = Registry::Get().Lookup(fn.name(), ptypes);
+    const FunctionDef* def = LookupFunction(fn.name(), ptypes);
     const DataType& rt = fn.return_type();
 
-    if (Val r; ViewShortcut(fn, out, indent, &r)) return r;
+    if (def->is_user()) EmitUserFunction(*def);
+    else if (Val r; ViewShortcut(fn, out, indent, &r)) return r;
 
     if (def->flags & kDateFormat) {
       Val s = Gen(*fn.children()[0], out, indent);
@@ -1200,9 +1214,29 @@ class BodyGen {
     call += ")";
 
     const std::string v = NewVar("v");
+    if (def->nulls != NullMode::kIfNull && (def->flags & kCanFail)) {
+      // sees nulls and can raise: called for every row of the batch (never for the padding of a tail)
+      std::string okv = "true";
+      if (def->nulls == NullMode::kInternal) {
+        okv = NewVar("ok");
+        *out += Ind(indent) + "bool " + okv + " = false;\n";
+        call.insert(call.size() - 1, ", &" + okv);
+      }
+      *out += Ind(indent) + rt.ctype() + " " + v + " = " + ZeroOf(rt) + ";\n";
+      *out += Ind(indent) + "if (in) " + v + " = " + call + ";\n";
+      return Val{v, okv, rt};
+    }
     if (def->nulls == NullMode::kNever) {
       *out += Ind(indent) + "const " + rt.ctype() + " " + v + " = " + call + ";\n";
       return Val{v, "true", rt};
+    }
+    if (def->nulls == NullMode::kInternal) {
+      // the function decides validity itself: it receives (value, valid) pairs and writes *out_valid
+      const std::string okv = NewVar("ok");
+      call.insert(call.size() - 1, ", &" + okv);
+      *out += Ind(indent) + "bool " + okv + " = false;\n";
+      *out += Ind(indent) + "const " + rt.ctype() + " " + v + " = " + call + ";\n";
+      return Val{v, okv, rt};
     }
     std::vector<std::string> oks;
     for (const auto& a : args) oks.push_back(a.ok);
@@ -1449,6 +1483,7 @@ class BodyGen {
   std::string error_;  // first construct the fuser cannot lower (reported by GenerateKernel)
   std::vector<CoopSeg> coop_segs_;
   std::string globals_;
+  std::vector<std::string> user_text_;  // preludes and user functions already in globals_
   struct ReplSite {
     std::string from, to;  // names of the literal byte arrays
     int fl, tl;

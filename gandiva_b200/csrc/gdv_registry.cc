@@ -1,8 +1,14 @@
 #include "gdv_registry.h"
 
+#include <cctype>
+#include <cstdio>
+
+#include "gdv_cuda.h"
+
 namespace gdv {
 
 std::string FunctionDef::device_name() const {
+  if (is_user()) return device_base;
   std::string s = device_base;
   for (const auto& p : params) {
     s += "_";
@@ -59,6 +65,177 @@ const FunctionDef* Registry::Lookup(const std::string& name,
 const Registry& Registry::Get() {
   static const Registry r;
   return r;
+}
+
+// ======================================================================================
+// User functions
+// ======================================================================================
+namespace {
+
+thread_local const FunctionRegistry* tl_user_functions = nullptr;
+
+bool IsUserValueType(const DataType& t, bool allow_varlen) {
+  if (t.is_dict() || t.is_view()) return false;
+  switch (t.id) {
+    case GDV_TYPE_BOOL: case GDV_TYPE_UINT8: case GDV_TYPE_INT8: case GDV_TYPE_UINT16: case GDV_TYPE_INT16:
+    case GDV_TYPE_UINT32: case GDV_TYPE_INT32: case GDV_TYPE_UINT64: case GDV_TYPE_INT64: case GDV_TYPE_FLOAT:
+    case GDV_TYPE_DOUBLE: case GDV_TYPE_DATE32: case GDV_TYPE_DATE64:
+      return true;
+    case GDV_TYPE_TIMESTAMP: case GDV_TYPE_TIME32: return t.precision == 1;  // milliseconds, as everywhere
+    case GDV_TYPE_STRING: case GDV_TYPE_BINARY: return allow_varlen;
+    default: return false;
+  }
+}
+
+const char* NullModeName(NullMode m) {
+  return m == NullMode::kIfNull ? "if_null" : m == NullMode::kNever ? "never" : "internal";
+}
+
+// The device function the fuser calls: the engine writes the signature in the convention built-ins of
+// the same null mode use (GenFunction), the caller supplies the statements.
+std::string UserFunctionText(const UserFunction& fn, const std::string& symbol, const std::string& signature) {
+  const bool pairs = fn.nulls != NullMode::kIfNull;
+  std::string t = "// user function: " + signature + " [" + NullModeName(fn.nulls) + (fn.can_raise ? ", can raise" : "") + "]\n";
+  t += std::string("__device__ __forceinline__ ") + fn.ret.ctype() + " " + symbol + "(";
+  bool first = true;
+  auto add = [&](const std::string& p) {
+    t += (first ? "" : ", ") + p;
+    first = false;
+  };
+  if (fn.can_raise) add("gdv_ctx* ctx");
+  for (size_t i = 0; i < fn.params.size(); ++i) {
+    const std::string n = std::to_string(i);
+    add(fn.params[i].is_varlen() ? "const gdv_str& a" + n : std::string(fn.params[i].ctype()) + " a" + n);
+    if (pairs) add("bool v" + n);
+  }
+  if (fn.nulls == NullMode::kInternal) add("bool* out_valid");
+  t += ") {\n" + fn.body;
+  if (fn.body.empty() || fn.body.back() != '\n') t += "\n";
+  return t + "}\n";
+}
+
+uint64_t Fnv1a64(const std::string& s) {
+  uint64_t h = 1469598103934665603ull;
+  for (unsigned char c : s) {
+    h ^= c;
+    h *= 1099511628211ull;
+  }
+  return h;
+}
+
+}  // namespace
+
+// ExecutionErrors with a caller's text: the lane that raises first writes the message behind the error
+// word (the engine's error block is 256 bytes) and the host reads it back with the code.  Written into a
+// kernel before its first user function that can raise.
+const char kUserRaiseHelper[] =
+    "#define GDV_ERR_USER 1000\n"
+    "__device__ __noinline__ void gdv_raise(gdv_ctx* c, const char* msg) {\n"
+    "  if (c->err == nullptr || atomicCAS(c->err, 0, GDV_ERR_USER) != 0) return;\n"
+    "  char* d = reinterpret_cast<char*>(c->err) + 8;\n"
+    "  int i = 0;\n"
+    "  for (; i < 239 && msg[i] != 0; ++i) d[i] = msg[i];\n"
+    "  d[i] = 0;\n"
+    "}\n";
+
+Status FunctionRegistry::Register(const UserFunction& fn) {
+  auto invalid = [](const std::string& m) { return Status::Make(GDV_INVALID, m); };
+  if (fn.name.empty() || !(std::isalpha(static_cast<unsigned char>(fn.name[0])) || fn.name[0] == '_'))
+    return invalid("user function name '" + fn.name + "' is not an identifier");
+  for (unsigned char c : fn.name)
+    if (!(std::isalnum(c) || c == '_')) return invalid("user function name '" + fn.name + "' is not an identifier");
+  FunctionDef d;
+  d.name = fn.name;
+  d.params = fn.params;
+  d.ret = fn.ret;
+  d.nulls = fn.nulls;
+  d.flags = fn.can_raise ? static_cast<uint32_t>(kCanFail) : 0u;
+  const std::string sig = d.signature();
+  for (const auto& p : fn.params) {
+    if (p.id == GDV_TYPE_DECIMAL128)
+      return Status::Make(GDV_NOT_IMPLEMENTED, "user function " + sig + ": decimal128 parameters are not supported");
+    if (!IsUserValueType(p, true)) return invalid("user function " + sig + ": unsupported parameter type " + p.ToString());
+  }
+  if (fn.ret.is_varlen() || fn.ret.id == GDV_TYPE_DECIMAL128)
+    return Status::Make(GDV_NOT_IMPLEMENTED, "user function " + sig + ": " + fn.ret.ToString() +
+                                                 " return types are not supported (fixed-width results only)");
+  if (!IsUserValueType(fn.ret, false)) return invalid("user function " + sig + ": unsupported return type " + fn.ret.ToString());
+  // The fuser recognises many built-ins by name (nvl, like, locate, equal over views, ...), so a built-in's
+  // name is taken for every parameter list, not only the ones it is defined for.
+  for (const auto& b : Registry::Get().all())
+    if (b.name == fn.name)
+      return invalid("user function " + sig + " clashes with the built-in function '" + fn.name +
+                     "': built-ins cannot be shadowed or overloaded");
+  if (fn.body.empty()) return invalid("user function " + sig + " has an empty body");
+
+  std::string hashed = sig + "|" + NullModeName(fn.nulls) + "|" + (fn.can_raise ? "1" : "0") + "|" + fn.prelude;
+  hashed.push_back('\0');
+  hashed += fn.body;
+  char hex[24];
+  std::snprintf(hex, sizeof(hex), "%016llx", static_cast<unsigned long long>(Fnv1a64(hashed)));
+  d.device_base = std::string("gdv_udf_") + hex;
+  d.prelude = fn.prelude;
+  if (!d.prelude.empty() && d.prelude.back() != '\n') d.prelude += "\n";
+  d.source = UserFunctionText(fn, d.device_base, sig);
+
+  std::lock_guard<std::mutex> lock(mu_);
+  if (frozen_)
+    return invalid("this function registry is already in use by a Projector or Filter: register every function "
+                   "before the first Make()");
+  if (Lookup(fn.name, fn.params) != nullptr) return invalid("user function " + sig + " is already registered");
+
+  // Probe: the prelude, the function and one kernel that calls it, with the options every kernel gets.
+  std::string probe = "#include \"gdv_device_lib.cuh\"\n";
+  if (fn.can_raise) probe += kUserRaiseHelper;
+  probe += d.prelude + d.source;
+  probe += "extern \"C\" __global__ void gdv_udf_probe(" + std::string(fn.ret.ctype()) + "* out, int* err) {\n";
+  if (fn.can_raise) probe += "  gdv_ctx ctx;\n  ctx.err = err;\n";
+  if (fn.nulls == NullMode::kInternal) probe += "  bool ov = false;\n";
+  probe += "  *out = " + d.device_base + "(";
+  bool first = true;
+  auto add = [&](const std::string& a) {
+    probe += (first ? "" : ", ") + a;
+    first = false;
+  };
+  if (fn.can_raise) add("&ctx");
+  for (const auto& p : fn.params) {
+    add(p.is_varlen() ? std::string("gdv_make_str(nullptr, 0)") : std::string("(") + p.ctype() + ")0");
+    if (fn.nulls != NullMode::kIfNull) add("true");
+  }
+  if (fn.nulls == NullMode::kInternal) add("&ov");
+  probe += ");\n}\n";
+  std::vector<char> cubin;
+  std::string log;
+  Status st = CompileToCubin(probe, "sm_90a", true, false, &cubin, nullptr, &log);
+  if (!st.ok()) {
+    if (st.code != GDV_CODEGEN_ERROR) return st;
+    return Status::Make(GDV_CODEGEN_ERROR, "user function " + sig + " does not compile:\n" + st.msg);
+  }
+  defs_.push_back(std::move(d));
+  return Status::OK();
+}
+
+void FunctionRegistry::Freeze() {
+  std::lock_guard<std::mutex> lock(mu_);
+  frozen_ = true;
+}
+
+const FunctionDef* FunctionRegistry::Lookup(const std::string& name, const std::vector<DataType>& params) const {
+  for (const auto& d : defs_) {
+    if (d.name != name || d.params.size() != params.size()) continue;
+    bool ok = true;
+    for (size_t i = 0; i < params.size() && ok; ++i) ok = ParamMatches(d.params[i], params[i]);
+    if (ok) return &d;
+  }
+  return nullptr;
+}
+
+FunctionRegistry::Scope::Scope(const FunctionRegistry* reg) : prev_(tl_user_functions) { tl_user_functions = reg; }
+FunctionRegistry::Scope::~Scope() { tl_user_functions = prev_; }
+
+const FunctionDef* LookupFunction(const std::string& name, const std::vector<DataType>& params) {
+  if (const FunctionDef* d = Registry::Get().Lookup(name, params)) return d;
+  return tl_user_functions != nullptr ? tl_user_functions->Lookup(name, params) : nullptr;
 }
 
 Registry::Registry() {

@@ -4,6 +4,8 @@
 // Device functions live in device/gdv_device_lib.cuh and are named
 // <base>_<suffix of each param>, the reference library's naming scheme.
 #pragma once
+#include <deque>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -38,6 +40,12 @@ struct FunctionDef {
   DataType ret;                   // decimal: precision/scale come from the call site
   NullMode nulls = NullMode::kIfNull;
   uint32_t flags = 0;
+  // User functions (FunctionRegistry) only: the file-scope text the caller supplied and the complete
+  // definition of the device function, written into every kernel that calls it.  device_base is then
+  // the whole symbol (gdv_udf_<hash>).
+  std::string prelude;
+  std::string source;
+  bool is_user() const { return !source.empty(); }
   std::string device_name() const;  // e.g. add_int32_int32
   std::string signature() const;    // "int32 add(int32, int32)"
 };
@@ -56,5 +64,60 @@ class Registry {
            const std::vector<std::string>& aliases = {});
   std::vector<FunctionDef> defs_;
 };
+
+struct Status;
+
+// What a caller hands to FunctionRegistry::Register: a signature plus the statements of the device
+// function (see include/gandiva_b200.h, gdv_function_def_t, for the calling convention).
+struct UserFunction {
+  std::string name;
+  std::vector<DataType> params;
+  DataType ret;
+  NullMode nulls = NullMode::kIfNull;
+  bool can_raise = false;
+  std::string body;
+  std::string prelude;
+};
+
+// Functions a caller adds to the engine: CUDA text that the fuser writes into the kernels that call it
+// (DESIGN.md §3.8).  A registry is scoped by the Config handed to Make(); the built-in table
+// (Registry::Get()) and its enumeration never change.
+//
+// Lifetime rule: Register() may be called until the first Make() that is given the registry; that Make()
+// freezes it (later Register() calls fail with GDV_INVALID).  A frozen registry is read without locks, so
+// any number of threads may Make() against it, and Projectors / Filters keep it alive.
+class FunctionRegistry {
+ public:
+  // Validates the definition and compiles it once with NVRTC for sm_90a (no GPU needed): a body that does
+  // not compile is refused here with GDV_CODEGEN_ERROR and NVRTC's log.
+  Status Register(const UserFunction& fn);
+  void Freeze();
+  const FunctionDef* Lookup(const std::string& name, const std::vector<DataType>& params) const;
+  const std::deque<FunctionDef>& all() const { return defs_; }
+
+  // Makes `reg` (may be null) the registry that LookupFunction() consults on this thread after the
+  // built-ins, for the lifetime of the object: validation and kernel generation run inside one.
+  class Scope {
+   public:
+    explicit Scope(const FunctionRegistry* reg);
+    ~Scope();
+    Scope(const Scope&) = delete;
+    Scope& operator=(const Scope&) = delete;
+
+   private:
+    const FunctionRegistry* prev_;
+  };
+
+ private:
+  mutable std::mutex mu_;
+  bool frozen_ = false;
+  std::deque<FunctionDef> defs_;  // a deque: definitions never move once a kernel plan points at them
+};
+
+// Text of gdv_raise(ctx, "message"), written into a kernel before its first user function that can raise.
+extern const char kUserRaiseHelper[];
+
+// Built-ins first, then the registry of the enclosing FunctionRegistry::Scope.
+const FunctionDef* LookupFunction(const std::string& name, const std::vector<DataType>& params);
 
 }  // namespace gdv

@@ -36,6 +36,18 @@ const char* ExecutionErrorMessage(int code) {
   }
 }
 
+// A user function raised (gdv_raise, kUserRaiseHelper): its message sits behind the error word of the
+// 256-byte error block.
+constexpr int kUserError = 1000;
+static std::string UserErrorText(CUdeviceptr d_err, CUstream stream) {
+  char text[248] = {0};
+  const DriverApi& d = Driver();
+  if (d.MemcpyDtoHAsync(text, d_err + 8, 240, stream) != CUDA_SUCCESS || d.StreamSynchronize(stream) != CUDA_SUCCESS ||
+      text[0] == 0)
+    return "error raised by a user function";
+  return text;
+}
+
 // ======================================================================================
 // Device
 // ======================================================================================
@@ -325,6 +337,7 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
   const std::string placeholder = std::string(KernelPrefix(kind)) + "PLACEHOLDER";
   spec.name = placeholder;
   std::unique_ptr<CompiledKernel> k(new CompiledKernel());
+  const FunctionRegistry::Scope user_functions(cfg.functions.get());
   GDV_RETURN_NOT_OK(GenerateKernel(schema, exprs, spec, &k->gen));
   // Compile for the device we will run on when one is visible, else for H100.
   std::string arch = "sm_90a";
@@ -713,6 +726,7 @@ Status Projector::Make(SchemaPtr schema, std::vector<ExpressionPtr> exprs, int s
                        const Config& cfg, std::shared_ptr<Projector>* out) {
   if (schema == nullptr) return Status::Make(GDV_INVALID, "Schema cannot be null");
   if (exprs.empty()) return Status::Make(GDV_INVALID, "Expressions cannot be empty");
+  const FunctionRegistry::Scope user_functions(cfg.functions.get());
   for (const auto& e : exprs) {
     if (e == nullptr) return Status::Make(GDV_INVALID, "Expression cannot be null");
     GDV_RETURN_NOT_OK(ValidateExpression(*schema, *e));
@@ -1322,13 +1336,15 @@ Status Projector::Sync(void* stream_v) {
       }
     }
   }
+  std::string user_text;
+  if (copy.ok() && s.ok() && err == kUserError) user_text = UserErrorText(pend.d_err, stream);
   if (have) {  // on every path: the pending blocks go back to the pool once the stream is idle
     if (pend.d_err != 0) dev->Free(pend.d_err);
     for (auto p : pend.scratch) dev->Free(p);
   }
   GDV_RETURN_NOT_OK(copy);
   GDV_RETURN_NOT_OK(s);
-  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, ExecutionErrorMessage(err) + detail);
+  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, (err == kUserError ? user_text : ExecutionErrorMessage(err)) + detail);
   return Status::OK();
 }
 
@@ -1339,6 +1355,7 @@ Status Filter::Make(SchemaPtr schema, ConditionPtr cond, const Config& cfg,
                     std::shared_ptr<Filter>* out) {
   if (schema == nullptr) return Status::Make(GDV_INVALID, "Schema cannot be null");
   if (cond == nullptr) return Status::Make(GDV_INVALID, "Condition cannot be null");
+  const FunctionRegistry::Scope user_functions(cfg.functions.get());
   GDV_RETURN_NOT_OK(ValidateExpression(*schema, *cond));
   std::shared_ptr<Filter> f(new Filter());
   f->schema_ = schema;
@@ -1660,13 +1677,15 @@ Status Filter::Sync(void* stream_v, int64_t* num_slots) {
   if (copy.ok() && have && pend.d_count != 0)
     copy = CuCheck(d.MemcpyDtoHAsync(&count, pend.d_count, sizeof(count), stream), "D2H count");
   Status s = CuCheck(d.StreamSynchronize(stream), "cuStreamSynchronize");
+  std::string user_text;
+  if (copy.ok() && s.ok() && err == kUserError) user_text = UserErrorText(pend.d_err, stream);
   if (have) {  // on every path: the pending blocks go back to the pool once the stream is idle
     if (pend.d_err != 0) dev->Free(pend.d_err);
     for (auto p : pend.scratch) dev->Free(p);
   }
   GDV_RETURN_NOT_OK(copy);
   GDV_RETURN_NOT_OK(s);
-  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, ExecutionErrorMessage(err));
+  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, err == kUserError ? user_text : ExecutionErrorMessage(err));
   if (num_slots != nullptr) *num_slots = have ? static_cast<int64_t>(count) : -1;
   return Status::OK();
 }

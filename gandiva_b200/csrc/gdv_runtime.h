@@ -14,6 +14,7 @@
 
 #include "gdv_codegen.h"
 #include "gdv_cuda.h"
+#include "gdv_registry.h"
 
 namespace gdv {
 
@@ -132,6 +133,9 @@ struct Config {
   int string_scan = 0;
   int filter_gating = 0;
   bool large_batch = false;  // set per kernel variant by Filter::KernelFor (batches >= 32 M rows)
+  // User functions looked up after the built-ins (frozen: see FunctionRegistry); null = none.  Kernel
+  // variants are compiled on first use, long after Make(), so the Projector / Filter keeps it alive.
+  std::shared_ptr<const FunctionRegistry> functions;
 };
 
 class CompiledKernel {

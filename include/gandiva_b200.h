@@ -111,6 +111,7 @@ typedef struct gdv_condition_s* gdv_condition_t;
 typedef struct gdv_schema_s* gdv_schema_t;
 typedef struct gdv_projector_s* gdv_projector_t;
 typedef struct gdv_filter_s* gdv_filter_t;
+typedef struct gdv_function_registry_s* gdv_function_registry_t;
 
 /* ---- configuration (gandiva::Configuration + device placement) --------- */
 typedef struct gdv_config {
@@ -137,7 +138,10 @@ typedef struct gdv_config {
   int32_t filter_gating;   /* fixed-width Filter: 0 = engine decides (gated loads wherever they apply: a
                               conjunct's columns are read only in rows the earlier conjuncts kept),
                               1 = off (every column read for every row; the reference kernel) */
-  int32_t reserved[2];
+  gdv_function_registry_t function_registry; /* user functions looked up after the built-ins (see
+                              gdv_function_registry_add); NULL = none.  These 8 bytes at offset 40 were
+                              `int32_t reserved[2]`: the struct keeps its size, and a caller that zeroes it or
+                              calls gdv_config_default keeps the built-in library only. */
 } gdv_config_t;
 void gdv_config_default(gdv_config_t* cfg);
 
@@ -356,6 +360,74 @@ int32_t gdv_registry_size(void);
 /* Signature i: name, return type, parameter types (up to max_params written; returns count). */
 gdv_status gdv_registry_get(int32_t i, const char** name, gdv_type_t* ret, gdv_type_t* params,
                             int32_t max_params, int32_t* n_params);
+
+/* ---- user-defined functions ----------------------------------------------------------------
+ * A function registry holds functions the caller adds to the engine as CUDA text.  A Projector or
+ * Filter made with gdv_config_t.function_registry set resolves a function name against the built-ins
+ * first and the registry second, and the fuser writes every user function a kernel calls into that
+ * kernel's source (gdv_*_dump_ir shows it), where NVRTC inlines it like a built-in.  The global
+ * enumeration above never changes.  User code runs inside the engine's kernels with the engine's
+ * privileges: a registry is for trusted callers, exactly like linking a library.
+ *
+ * The caller writes the statements of the function; the engine writes the signature.
+ *   - parameter i is `a<i>`: bool, i8..i64 / u8..u64, f32, f64 (date32 / time32 are i32; date64 /
+ *     timestamp are i64), `const gdv_str&` for utf8 / binary: s.len bytes, byte i is gdv_ch(s, i)
+ *     (never s.p[i]: upper / lower / initcap views re-case bytes as they are read).  The same text
+ *     serves plain, sliced, dictionary-encoded and string_view / binary_view columns.
+ *   - GDV_NULL_IF_NULL  T f(a0, a1, ...)                     result is null iff an argument is null;
+ *                                                            arguments of null rows are unspecified
+ *   - GDV_NULL_NEVER    T f(a0, bool v0, a1, bool v1, ...)   v<i> = argument i is valid; never null
+ *   - GDV_NULL_INTERNAL T f(a0, bool v0, ..., bool* out_valid)   *out_valid (preset to false) = result
+ *                                                            is valid
+ *   - can_raise: `gdv_ctx* ctx` comes first; gdv_raise(ctx, "message") makes the evaluation fail with
+ *     GDV_EXECUTION_ERROR and that message (at most 239 bytes; the first raise wins).  Such a function
+ *     is called only for rows of the batch that reach it (not in the untaken branch of an if, not
+ *     past a decided and / or), and with GDV_NULL_IF_NULL only where every argument is valid.
+ *   - prelude: file-scope text written once before the function (helpers, __constant__ tables).
+ * Types: fixed-width parameters and results, utf8 / binary parameters.  utf8 / binary / decimal128
+ * results and decimal128 parameters are refused with GDV_NOT_IMPLEMENTED.  A built-in's name cannot
+ * be reused, whatever the parameter types.  Everything is compiled with --fmad=false like the
+ * engine's own code.
+ *
+ * gdv_function_registry_add validates and compiles the function once for sm_90a (no GPU needed): text
+ * that does not compile is refused there with GDV_CODEGEN_ERROR and NVRTC's log in gdv_last_error().
+ * Functions can be added until the first gdv_projector_make / gdv_filter_make that is given the
+ * registry; from then on the registry is read-only (add fails with GDV_INVALID) and may be shared by
+ * any number of threads.  Projectors and Filters keep what they need: the handle may be released
+ * while they live.
+ *
+ *   gdv_function_registry_t reg;
+ *   gdv_function_registry_create(&reg);
+ *   gdv_type_t f64 = {GDV_TYPE_DOUBLE, 0, 0};
+ *   gdv_function_def_t def = {0};
+ *   def.name = "fahrenheit";  def.params = &f64;  def.n_params = 1;  def.ret = f64;
+ *   def.null_mode = GDV_NULL_IF_NULL;
+ *   def.body = "return a0 * 1.8 + 32.0;";
+ *   gdv_function_registry_add(reg, &def);
+ *   gdv_config_t cfg;  gdv_config_default(&cfg);  cfg.function_registry = reg;
+ *   // gdv_node_function("fahrenheit", &celsius, 1, f64, &node) ... gdv_projector_make(..., &cfg, &p)
+ */
+#define GDV_NULL_IF_NULL 0
+#define GDV_NULL_NEVER 1
+#define GDV_NULL_INTERNAL 2
+typedef struct gdv_function_def {
+  const char* name;
+  const gdv_type_t* params;
+  int32_t n_params;
+  gdv_type_t ret;
+  int32_t null_mode; /* GDV_NULL_* */
+  int32_t can_raise;
+  const char* body;
+  const char* prelude; /* may be NULL */
+} gdv_function_def_t;
+gdv_status gdv_function_registry_create(gdv_function_registry_t* out);
+void gdv_function_registry_release(gdv_function_registry_t reg);
+gdv_status gdv_function_registry_add(gdv_function_registry_t reg, const gdv_function_def_t* def);
+/* Enumeration of this registry only: gdv_function_registry_signatures returns the count; signature i
+ * as in gdv_registry_get. */
+int32_t gdv_function_registry_signatures(gdv_function_registry_t reg);
+gdv_status gdv_function_registry_get(gdv_function_registry_t reg, int32_t i, const char** name, gdv_type_t* ret,
+                                     gdv_type_t* params, int32_t max_params, int32_t* n_params);
 
 /* ---- device memory (the engine's pooled allocator; what the C++ layer's arrow::MemoryManager
  *      for HBM, include/gandiva/device.h, allocates from) ---------------------------------- */
