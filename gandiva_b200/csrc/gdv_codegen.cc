@@ -572,30 +572,16 @@ class BodyGen {
   }
 
   static bool CanFail(const Node& node) {
-    switch (node.kind()) {
-      case NodeKind::kField: case NodeKind::kLiteral: return false;
-      case NodeKind::kFunction: {
-        const auto& fn = static_cast<const FunctionNode&>(node);
-        std::vector<DataType> params;
-        for (const auto& c : fn.children()) params.push_back(c->return_type());
-        const FunctionDef* def = LookupFunction(fn.name(), params);
-        if (def != nullptr && (def->flags & kCanFail)) return true;
-        if (ArgGuard(fn) >= 0) return true;
-        for (const auto& c : fn.children())
-          if (CanFail(*c)) return true;
-        return false;
-      }
-      case NodeKind::kIf: {
-        const auto& n = static_cast<const IfNode&>(node);
-        return CanFail(*n.condition()) || CanFail(*n.then_node()) || CanFail(*n.else_node());
-      }
-      case NodeKind::kBoolean: {
-        for (const auto& c : static_cast<const BooleanNode&>(node).children())
-          if (CanFail(*c)) return true;
-        return false;
-      }
-      case NodeKind::kIn: return CanFail(*static_cast<const InNode&>(node).child());
+    if (node.kind() == NodeKind::kFunction) {
+      const auto& fn = static_cast<const FunctionNode&>(node);
+      std::vector<DataType> params;
+      for (const auto& c : fn.children()) params.push_back(c->return_type());
+      const FunctionDef* def = LookupFunction(fn.name(), params);
+      if (def != nullptr && (def->flags & kCanFail)) return true;
+      if (ArgGuard(fn) >= 0) return true;
     }
+    for (const auto& c : Children(node))
+      if (CanFail(*c)) return true;
     return false;
   }
 
@@ -1538,8 +1524,9 @@ const char* SelCType(int mode) {
 
 // ---- kernel skeleton pieces ------------------------------------------------------------
 // Hoisted, typed views of the argument block (read once per thread, live in registers /
-// uniform registers for the whole kernel).
-void EmitPrologue(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, std::string* o) {
+// uniform registers for the whole kernel), and `sel` when the kernel reads its rows through a
+// selection vector (`has_sel`).
+void EmitPrologue(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, bool has_sel, std::string* o) {
   for (size_t j = 0; j < slots.size(); ++j) {
     const DataType& t = slots[j].type;
     const std::string J = std::to_string(j);
@@ -1577,14 +1564,15 @@ void EmitPrologue(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, 
       *o += "  const i64 in_vm" + J + " = in_hv" + J + " ? -1ll : 0ll;\n";
     }
   }
-  if (spec.kind == KernelKind::kProject && spec.selection_mode != GDV_SEL_NONE)
+  if (has_sel)
     *o += "  const " + std::string(SelCType(spec.selection_mode)) +
           "* sel = reinterpret_cast<const " + SelCType(spec.selection_mode) + "*>(A.sel);\n";
 }
 
 // One group of R steps (32 rows each) starting at row `base` (a multiple of 32):
 // declarations, load phase, then the compute loop whose per-step tail is `step_tail`
-// (stores / ballots; may use `s`, `in`, `k`).  `fast` = every row of the group is in range
+// (stores / ballots; may use `s`, `in`, `k`).  `has_sel`: row s of the group is row sel[s] of the
+// batch (a projector given a selection vector).  `fast` = every row of the group is in range
 // and rows are contiguous (no selection vector): loads are unconditional, back to back, with
 // immediate offsets from one pointer per column; validity arrives as one 32-bit window per
 // step (a warp-uniform load) instead of one byte load per row.
@@ -1759,14 +1747,13 @@ bool SlotHasCoop(const std::vector<CoopSeg>& segs, int j) {
   return false;
 }
 
-void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int R, int mode,
+void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, bool has_sel, int R, int mode,
                const std::string& body, const std::string& step_tail, std::string* o, int indent,
                int stage_bytes = 0, const std::string& after_loads = std::string(),
                const std::vector<CoopSeg>& coop = std::vector<CoopSeg>(), bool prefetched = false) {
   const bool fast = mode != kPred;
   const std::string I(static_cast<size_t>(indent) * 2, ' ');
   const std::string sR = std::to_string(R);
-  const bool has_sel = spec.kind == KernelKind::kProject && spec.selection_mode != GDV_SEL_NONE;
   for (size_t j = 0; j < slots.size(); ++j) {
     const DataType& t = slots[j].type;
     *o += I + t.ctype() + " f" + std::to_string(j) + "[" + sR + "];\n";
@@ -2247,7 +2234,7 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
   // the condition of ONE row per lane: EmitGroup's per-row path with `base` chosen so that row s is
   // the anchor's row (lanes without one get s = A.n, i.e. out of range)
   std::string pred;
-  EmitGroup(slots, spec, 1, kPred, body,
+  EmitGroup(slots, spec, false, 1, kPred, body,
             "              { keep = in && (" + result.ok + ") && (" + result.v + "); }\n", &pred, 7);
   std::string k = mk + R"K(extern "C" __global__ void __launch_bounds__(@BT@, @MINB@) @NAME@(const __grid_constant__ gdv_args A) {
   const u32 lane = threadIdx.x & 31u;
@@ -2433,7 +2420,7 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
     verify += "            }\n";
   }
   std::string prologue, epilogue;
-  EmitPrologue(slots, spec, &prologue);
+  EmitPrologue(slots, spec, false, &prologue);
   prologue += scratch_decl;
   EmitFilterEpilogue(slots, spec, NW, W, SelCType(spec.selection_mode), &epilogue);
   ReplaceAll(&k, "@PROLOGUE@", prologue);
@@ -2489,25 +2476,13 @@ void MarkHoisted(const BodyGen& gen, const Node& cond, std::vector<ColumnSlot>* 
       sl.hoist = true;
 }
 
-void CollectFields(const Schema& schema, const Node& node, std::vector<int>* cols) {
-  switch (node.kind()) {
-    case NodeKind::kField: cols->push_back(schema.index_of(static_cast<const FieldNode&>(node).name())); return;
-    case NodeKind::kLiteral: return;
-    case NodeKind::kFunction:
-      for (const auto& c : static_cast<const FunctionNode&>(node).children()) CollectFields(schema, *c, cols);
-      return;
-    case NodeKind::kIf: {
-      const auto& n = static_cast<const IfNode&>(node);
-      CollectFields(schema, *n.condition(), cols);
-      CollectFields(schema, *n.then_node(), cols);
-      CollectFields(schema, *n.else_node(), cols);
-      return;
-    }
-    case NodeKind::kBoolean:
-      for (const auto& c : static_cast<const BooleanNode&>(node).children()) CollectFields(schema, *c, cols);
-      return;
-    case NodeKind::kIn: CollectFields(schema, *static_cast<const InNode&>(node).child(), cols); return;
+// The schema columns a tree reads, each once, in the order of their first use.
+void CollectColumns(const Schema& schema, const Node& node, std::vector<int>* cols) {
+  if (node.kind() == NodeKind::kField) {
+    const int i = schema.index_of(static_cast<const FieldNode&>(node).name());
+    if (std::find(cols->begin(), cols->end(), i) == cols->end()) cols->push_back(i);
   }
+  for (const auto& c : Children(node)) CollectColumns(schema, *c, cols);
 }
 
 void SpineConjuncts(const Node& node, std::vector<const Node*>* out) {
@@ -2532,7 +2507,7 @@ bool PlanGate(const Schema& schema, const Node& cond, const std::vector<ColumnSl
   std::vector<int> level(conj.size(), 0);
   for (size_t c = 0; c < conj.size(); ++c) {
     std::vector<int> cols;
-    CollectFields(schema, *conj[c], &cols);
+    CollectColumns(schema, *conj[c], &cols);
     for (int col : cols) {
       int j = -1;
       for (size_t s = 0; s < slots.size(); ++s)
@@ -2577,6 +2552,123 @@ int PickRowsPerThread(int in_bytes, int out_bytes, KernelKind kind) {
   return p;
 }
 
+// ---- pieces every kernel generator shares -------------------------------------------------------
+// A BodyGen over `slots` as `spec` configures it: string_scan bit 0 turns the cooperative LIKE scan
+// off, bit 3 the inline / prefix shortcut over string_view / binary_view views.
+BodyGen SpecBodyGen(const Schema& schema, std::vector<ColumnSlot>* slots, const KernelSpec& spec) {
+  return BodyGen(schema, slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
+}
+
+// Algorithmic bytes (values only) a kernel over `slots` reads per row.
+int InBytesPerRow(const std::vector<ColumnSlot>& slots) {
+  int bytes = 0;
+  for (const auto& s : slots)
+    bytes += s.type.is_dict() ? DataType(s.type.index).width()  // the index; the dictionary is cached
+             : s.type.is_view()   ? 16                               // the view; out-of-line bytes on demand
+             : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);  // 4 B offset + ~28 B data
+  return bytes;
+}
+
+// The fields of `out` that follow from the spec and the kernel's input slots, among them the layout
+// of the argument block the kernel is emitted with and the host packs.
+void DescribeKernel(const KernelSpec& spec, const std::vector<ColumnSlot>& slots, int n_out, GeneratedKernel* out) {
+  out->name = spec.name;
+  out->kind = spec.kind;
+  out->selection_mode = spec.selection_mode;
+  out->nullable = spec.nullable;
+  out->inputs = slots;
+  out->in_bytes_per_row = InBytesPerRow(slots);
+  out->args = ArgsLayout(static_cast<int>(slots.size()), n_out, HasDictionary(slots), HasView(slots));
+}
+
+// The comment lines a kernel's source starts with.
+std::string HeaderLines(const std::string& shape, const KernelSpec& spec, const std::vector<ExpressionPtr>& exprs) {
+  std::string h = "// generated by gandiva_b200 kernel fuser; " + shape;
+  h += spec.nullable ? " (inputs may carry validity bitmaps)\n" : " (no input has nulls)\n";
+  for (size_t i = 0; i < exprs.size(); ++i)
+    h += "// expr_" + std::to_string(i) + ": " + CommentSafe(exprs[i]->ToString()) + "\n";
+  return h;
+}
+
+// A kernel's text up to its loops: the `header` lines, the device library, the argument block of
+// `out`, the globals of `gen`, the signature with launch bounds `bounds`, lane / wid / ctx, the
+// prologue and the scratch of `gen` for out.rows_per_thread rows per group.
+std::string EmitKernelFrame(const KernelSpec& spec, bool has_sel, const GeneratedKernel& out, const BodyGen& gen,
+                            const std::string& header, const std::string& bounds) {
+  std::string src = header;
+  src += "#include \"gdv_device_lib.cuh\"\n";
+  src += EmitArgsStruct(out.args);
+  src += gen.globals();
+  src += "extern \"C\" __global__ void __launch_bounds__(" + bounds + ") " + spec.name +
+         "(const __grid_constant__ gdv_args A) {\n";
+  src += "  const u32 lane = threadIdx.x & 31u;\n";
+  src += "  const u32 wid = threadIdx.x >> 5;\n";
+  src += "  gdv_ctx ctx;\n  ctx.err = A.err;\n";
+  EmitPrologue(out.inputs, spec, has_sel, &src);
+  src += gen.ScratchDecl(out.rows_per_thread);
+  return src;
+}
+
+// Shared memory of the string columns (HasByteRun), per warp and column: `stages` stages of 48 B
+// per row of a group, then the hit list and counters of the cooperative scan.
+struct StringStages {
+  int columns = 0;
+  int stages = 1;
+  int stage_bytes = 0;
+  int hit_bytes = 0;  // candidates, hits, two counters
+  int block() const { return stages * stage_bytes + hit_bytes; }
+  int dynamic_smem(int BT) const { return block() * (BT / 32) * columns; }
+};
+
+// Block size and string stages of a row-driven kernel over `slots` with R rows per thread.  Many
+// string columns (e.g. a schema extended by materialised ropes, gdv_rope_temps.h): the per-warp stages
+// of all of them must fit the CTA's shared memory — fewer rows per thread first, then fewer warps per CTA.
+Status FitStages(const KernelSpec& spec, const BodyGen& gen, const std::vector<ColumnSlot>& slots, int n_stages,
+                 int* R, int* BT, StringStages* st) {
+  int n_varlen = 0;
+  for (const auto& s : slots) n_varlen += HasByteRun(s) ? 1 : 0;
+  // String predicates are instruction-bound and stage bytes per warp in shared memory: they run
+  // 512 threads on big batches; everything else runs 256.
+  *BT = spec.block_threads > 0 ? spec.block_threads
+                               : (spec.kind == KernelKind::kFilter && n_varlen > 0 && spec.large_batch ? 512 : 256);
+  if (*BT % 32 != 0 || *BT > 1024)
+    return Status::Make(GDV_INVALID, "block_threads must be a multiple of 32 and <= 1024");
+  const int hit = gen.coop_segs().empty() ? 0 : 8 * kHitCap + 16;
+  auto need = [&](int r, int bt) { return (n_stages * 48 * 32 * r + hit) * (bt / 32) * n_varlen; };
+  const int kMaxStage = 200 * 1024;
+  while (need(*R, *BT) > kMaxStage && *R > 1) *R /= 2;
+  while (need(*R, *BT) > kMaxStage && *BT > 64 && spec.block_threads == 0) *BT /= 2;
+  if (need(*R, *BT) > kMaxStage)
+    return Status::Make(GDV_NOT_IMPLEMENTED, "too many utf8/binary columns for one kernel (" + std::to_string(n_varlen) + ")");
+  st->columns = n_varlen;
+  st->stages = n_stages;
+  st->stage_bytes = n_varlen > 0 ? 48 * 32 * *R : 0;
+  st->hit_bytes = hit;
+  return Status::OK();
+}
+
+// Warp `wid`'s stage of every string column (`decl` stage<j><suffix>) and, for the columns the
+// cooperative scan reads, its hit list and counters (hctr<j> ... `hctr_end`).
+std::string EmitStageDecls(const std::vector<ColumnSlot>& slots, const std::vector<CoopSeg>& coop,
+                           const StringStages& st, const std::string& decl, const std::string& suffix,
+                           const std::string& hctr_end) {
+  std::string o = "  extern __shared__ uint4 gdv_smem[];\n";
+  int vi = 0;
+  for (size_t j = 0; j < slots.size(); ++j) {
+    if (!HasByteRun(slots[j])) continue;
+    const std::string J = std::to_string(j), SJ = "stage" + J + suffix;
+    o += "  " + decl + SJ + " = reinterpret_cast<u8*>(gdv_smem) + ((size_t)wid * " + std::to_string(st.columns) +
+         " + " + std::to_string(vi) + ") * " + std::to_string(st.block()) + ";\n";
+    if (SlotHasCoop(coop, static_cast<int>(j))) {
+      o += "  u32* cand" + J + " = reinterpret_cast<u32*>(" + SJ + " + " + std::to_string(st.stages * st.stage_bytes) + ");\n";
+      o += "  u32* hits" + J + " = cand" + J + " + " + std::to_string(kHitCap) + ";\n";
+      o += "  u32* hctr" + J + " = hits" + J + " + " + std::to_string(kHitCap) + hctr_end;
+    }
+    ++vi;
+  }
+  return o;
+}
+
 // ---- string-producing projections ---------------------------------------------------------------
 // One utf8/binary output expression = two kernels around a tile scan (DESIGN.md "String outputs"):
 //   gdv_strsize_*  : bytes produced by every CTA tile -> tile_state[tile]
@@ -2590,76 +2682,27 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
                             GeneratedKernel* out) {
   const bool is_size = spec.kind == KernelKind::kStringSize;
   std::vector<ColumnSlot> slots;
-  BodyGen gen(schema, &slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
+  BodyGen gen = SpecBodyGen(schema, &slots, spec);
   std::string body;
   const Val res = gen.Gen(*expr->root(), &body, 4);
   if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
-  int n_varlen = 0, in_bytes = 0;
-  for (const auto& s : slots) {
-    n_varlen += HasByteRun(s) ? 1 : 0;
-    in_bytes += s.type.is_view() ? 16 : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);
-  }
   int R = spec.rows_per_thread > 0 ? std::min(spec.rows_per_thread, 8) : 2;
-  // String predicates are instruction-bound and stage bytes per warp in shared memory: they run
-  // 512 threads on big batches; everything else runs 256.
-  int BT = spec.block_threads > 0 ? spec.block_threads
-                                  : (spec.kind == KernelKind::kFilter && n_varlen > 0 && spec.large_batch ? 512 : 256);
-  if (BT % 32 != 0 || BT > 1024)
-    return Status::Make(GDV_INVALID, "block_threads must be a multiple of 32 and <= 1024");
-  {  // many string columns: the per-warp stages of all of them must fit the CTA's shared memory
-    const int hit = gen.coop_segs().empty() ? 0 : 8 * kHitCap + 16;
-    auto need = [&](int r, int bt) { return (48 * 32 * r + hit) * (bt / 32) * n_varlen; };
-    const int kMaxStage = 200 * 1024;
-    while (need(R, BT) > kMaxStage && R > 1) R /= 2;
-    while (need(R, BT) > kMaxStage && BT > 64 && spec.block_threads == 0) BT /= 2;
-    if (need(R, BT) > kMaxStage)
-      return Status::Make(GDV_NOT_IMPLEMENTED, "too many utf8/binary columns for one kernel (" + std::to_string(n_varlen) + ")");
-  }
+  int BT = 0;
+  StringStages st;
+  const Status fit = FitStages(spec, gen, slots, 1, &R, &BT, &st);
+  if (!fit.ok()) return fit;
   const int NW = BT / 32;
   const int T = BT * R;
-  const int stage_bytes = n_varlen > 0 ? 48 * 32 * R : 0;
-  const std::vector<CoopSeg>& coop = gen.coop_segs();
-  const int hit_bytes = coop.empty() ? 0 : 8 * kHitCap + 16;
-  const int col_block = stage_bytes + hit_bytes;
-  const int dynamic_smem = col_block * NW * n_varlen;
   const bool has_sel = spec.selection_mode != GDV_SEL_NONE;
-  ArgsLayout L(static_cast<int>(slots.size()), 1, HasDictionary(slots), HasView(slots));
+  DescribeKernel(spec, slots, 1, out);
+  out->rows_per_thread = R;
+  out->block_threads = BT;
   const std::string sR = std::to_string(R), s32R = std::to_string(32 * R), sT = std::to_string(T);
 
-  std::string src;
-  src += std::string("// generated by gandiva_b200 kernel fuser; string projection, ") +
-         (is_size ? "sizing pass" : "write pass") +
-         (spec.nullable ? " (inputs may carry validity bitmaps)\n" : " (no input has nulls)\n");
-  src += "// expr_0: " + CommentSafe(expr->ToString()) + "\n";
-  if (gen.has_replace()) src += "#define GDV_HAS_REPL 1\n";
-  src += "#include \"gdv_device_lib.cuh\"\n";
-  src += EmitArgsStruct(L);
-  src += gen.globals();
-  src += "extern \"C\" __global__ void __launch_bounds__(" + std::to_string(BT) + ") " + spec.name +
-         "(const __grid_constant__ gdv_args A) {\n";
-  src += "  const u32 lane = threadIdx.x & 31u;\n";
-  src += "  const u32 wid = threadIdx.x >> 5;\n";
-  src += "  gdv_ctx ctx;\n  ctx.err = A.err;\n";
-  KernelSpec pspec = spec;
-  pspec.kind = KernelKind::kProject;  // prologue / group emitters key on project vs filter only
-  EmitPrologue(slots, pspec, &src);
-  src += gen.ScratchDecl(R);
-  if (stage_bytes > 0) {
-    src += "  extern __shared__ uint4 gdv_smem[];\n";
-    int vi = 0;
-    for (size_t j = 0; j < slots.size(); ++j) {
-      if (!HasByteRun(slots[j])) continue;
-      const std::string J = std::to_string(j);
-      src += "  u8* stage" + J + " = reinterpret_cast<u8*>(gdv_smem) + ((size_t)wid * " +
-             std::to_string(n_varlen) + " + " + std::to_string(vi) + ") * " + std::to_string(col_block) + ";\n";
-      if (SlotHasCoop(coop, static_cast<int>(j))) {
-        src += "  u32* cand" + J + " = reinterpret_cast<u32*>(stage" + J + " + " + std::to_string(stage_bytes) + ");\n";
-        src += "  u32* hits" + J + " = cand" + J + " + " + std::to_string(kHitCap) + ";\n";
-        src += "  u32* hctr" + J + " = hits" + J + " + " + std::to_string(kHitCap) + ";\n";
-      }
-      ++vi;
-    }
-  }
+  std::string header = HeaderLines(is_size ? "string projection, sizing pass" : "string projection, write pass", spec, {expr});
+  if (gen.has_replace()) header += "#define GDV_HAS_REPL 1\n";
+  std::string src = EmitKernelFrame(spec, has_sel, *out, gen, header, std::to_string(BT));
+  if (st.stage_bytes > 0) src += EmitStageDecls(slots, gen.coop_segs(), st, "u8* ", "", ";\n");
   src += "  __shared__ u64 s_part[" + std::to_string(NW) + "];\n";
   if (has_sel && !is_size)  // a device count of 0 leaves no tile to write offsets[0]
     src += "  if (A.n == 0 && blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<i32*>(A.out_val[0])[0] = 0;\n";
@@ -2686,13 +2729,13 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   }
   if (!has_sel) {
     src += "    if (base + " + s32R + " <= A.n) {\n";
-    EmitGroup(slots, pspec, R, kFast, body, tail, &src, 3, stage_bytes, std::string(), coop);
+    EmitGroup(slots, spec, has_sel, R, kFast, body, tail, &src, 3, st.stage_bytes, std::string(), gen.coop_segs());
     src += "    } else {\n";
-    EmitGroup(slots, pspec, R, kPred, body, tail, &src, 3, 0, std::string(), coop);
+    EmitGroup(slots, spec, has_sel, R, kPred, body, tail, &src, 3, 0, std::string(), gen.coop_segs());
     src += "    }\n";
   } else {
     src += "    {\n";
-    EmitGroup(slots, pspec, R, kPred, body, tail, &src, 3, 0, std::string(), coop);
+    EmitGroup(slots, spec, has_sel, R, kPred, body, tail, &src, 3, 0, std::string(), gen.coop_segs());
     src += "    }\n";
   }
   if (is_size) {
@@ -2780,23 +2823,500 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   if (has_sel) ApplyDeviceCount(&src);
 
   out->source = std::move(src);
-  out->name = spec.name;
-  out->kind = spec.kind;
-  out->rows_per_thread = R;
-  out->block_threads = BT;
-  out->selection_mode = spec.selection_mode;
-  out->nullable = spec.nullable;
-  out->inputs = slots;
   out->outputs = {expr->result().type};
   out->uses_ctx = gen.uses_ctx() || !is_size;
-  out->in_bytes_per_row = in_bytes;
   out->out_bytes_per_row = 4;
-  out->args_size = L.size;
-  out->dynamic_smem = dynamic_smem;
+  out->dynamic_smem = st.dynamic_smem(BT);
   out->tile_rows = T;
-  out->staged = false;
-  out->stages = 0;
   out->cta_tile_rows = T;
+  out->view_shortcuts = gen.view_shortcuts();
+  return Status::OK();
+}
+
+// ---- key-driven string Filter -------------------------------------------------------------------
+// Default wherever it applies (string_scan bit 2 keeps the row-driven kernel): driven by the
+// occurrences of a literal of the condition in the column's bytes.  Conditions that can raise keep
+// the row-driven kernel so that errors come from the same rows.  False, with `out` untouched, where
+// it does not apply.
+bool GenerateKeyFilter(const Schema& schema, const std::vector<ExpressionPtr>& exprs, const KernelSpec& spec,
+                       GeneratedKernel* out) {
+  if ((spec.string_scan & 4) != 0 || exprs.size() != 1 || BodyGen::CanFail(*exprs[0]->root())) return false;
+  std::vector<ColumnSlot> kslots;
+  BodyGen kgen(schema, &kslots, spec.nullable, /*coop=*/false);
+  KeyPlan plan;
+  const int kBT = spec.block_threads > 0 ? spec.block_threads : 256;
+  // chunks of 1024 rows per warp and tile: more rows per anchor drain and per tile-end barrier on
+  // big batches (Configuration.stages overrides), one on small ones (enough tiles for 132 SMs)
+  const int kW = (spec.stages == 1 || spec.stages == 2 || spec.stages == 4) ? spec.stages : (spec.large_batch ? 2 : 1);
+  if (kBT % 32 != 0 || kBT > 1024 || !kgen.PlanKey(*exprs[0]->root(), &plan)) return false;
+  std::string kbody;
+  const Val kres = kgen.GenTruth(*exprs[0]->root(), &kbody, 6);
+  // the anchor drain loads rows one by one from plain columns only
+  if (!kgen.error().empty() || kgen.uses_ctx() || HasDictionary(kslots) || HasView(kslots)) return false;
+  if (spec.nullable) MarkHoisted(kgen, *exprs[0]->root(), &kslots);
+  DescribeKernel(spec, kslots, 0, out);
+  std::string src = HeaderLines("key-driven string Filter", spec, exprs);
+  src += "// key: '" + CommentSafe(plan.key) + "' in column slot " + std::to_string(plan.slot) +
+         ", case map " + std::to_string(plan.xf) + "\n";
+  src += "#include \"gdv_device_lib.cuh\"\n";
+  src += EmitArgsStruct(out->args);
+  src += kgen.globals();
+  src += EmitKeyFilter(kslots, spec, plan, kbody, kres, kBT, kW, kgen.ScratchDecl(1));
+  out->source = std::move(src);
+  out->rows_per_thread = 1;
+  out->block_threads = kBT;
+  out->dynamic_smem = (kBT / 32) * (kKeyAnchorCap + 32 * kW + 4) * 4;
+  out->tile_rows = static_cast<int64_t>(kBT / 32) * 1024 * kW;
+  out->key_driven = true;
+  return true;
+}
+
+// ---- row-driven Filter --------------------------------------------------------------------------
+// Fixed-width columns.  Every warp walks W consecutive 1024-row chunks per tile, so a 32K-row tile
+// needs 256 threads at W = 4 and eight small CTAs share an SM: while one sits in its tile-end
+// barriers and look-back, seven keep streaming.  Gated loads (EmitGatedGroup) where `gate_seg` is
+// not empty.
+void EmitChunkLoop(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int R, int W, const std::string& body,
+                   const std::string& step_tail, const std::vector<CoopSeg>& coop, const GatePlan& gate,
+                   const std::vector<std::string>& gate_seg, std::string* o) {
+  std::string& src = *o;
+  const std::string sR = std::to_string(R), s32R = std::to_string(32 * R);
+  const bool gated = !gate_seg.empty();
+  src += "    #pragma unroll\n";
+  src += "    for (int w = 0; w < " + std::to_string(W) + "; ++w) {\n";
+  src += "      const i64 wbase = wbase0 + 1024 * w;\n";
+  src += "      u32 cur = 0u;\n";
+  src += "      #pragma unroll 1\n";
+  src += "      for (int g = 0; g < 32; g += " + sR + ") {\n";
+  src += "        const i64 base = wbase + 32 * g;\n";
+  src += "        if (base >= A.n) break;\n";
+  src += "        if (base + " + s32R + " <= A.n) {\n";
+  const std::string gated_tail =
+      "          { const u32 m = __ballot_sync(GDV_FULL, in && alive[k]); if (lane == (u32)(g + k)) cur = m; }\n";
+  if (gated)
+    EmitGatedGroup(slots, spec, R, kFast, gate, gate_seg, gated_tail, &src, 5);
+  else
+    EmitGroup(slots, spec, false, R, kFast, body, step_tail, &src, 5, 0, std::string(), coop);
+  src += "        } else {\n";
+  if (gated)
+    EmitGatedGroup(slots, spec, R, kPred, gate, gate_seg, gated_tail, &src, 5);
+  else
+    EmitGroup(slots, spec, false, R, kPred, body, step_tail, &src, 5, 0, std::string(), coop);
+  src += "        }\n";
+  src += "      }\n";
+  src += "      mymask[w] = cur;\n";
+  src += "    }\n";
+}
+
+// String columns: one 1024-row chunk per warp; the bytes of the NEXT group are copied into a
+// second shared-memory stage with cp.async while the current group is scanned.
+void EmitPrefetchLoop(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, int R, int stage_bytes,
+                      const std::string& body, const std::string& step_tail, const std::vector<CoopSeg>& coop,
+                      std::string* o) {
+  std::string& src = *o;
+  const std::string sR = std::to_string(R), s32R = std::to_string(32 * R);
+  src += "    const i64 wbase = wbase0;\n";
+  src += "    u32 cur = 0u;\n";
+  // issue(b, par): cp.async the bytes of the full group that starts at row b into stage `par`
+  src += "    auto issue = [&](i64 b, u32 par) {\n";
+  for (size_t j = 0; j < slots.size(); ++j) {
+    if (!HasByteRun(slots[j])) continue;
+    const std::string J = std::to_string(j);
+    src += "      {\n";
+    src += "        const i32 gb = in_val" + J + "[b];\n";
+    src += "        const i32 gn = in_val" + J + "[b + " + s32R + "] - gb;\n";
+    src += "        const u8* src = in_var" + J + " + gb;\n";
+    src += "        const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
+    src += "        if (gn + (i32)mis <= " + std::to_string(stage_bytes) + ") {\n";
+    src += "          const i32 nchunks = (gn + (i32)mis + 15) >> 4;\n";
+    src += "          u8* dst = stage" + J + "_0 + (size_t)par * " + std::to_string(stage_bytes) + "u;\n";
+    src += "          for (i32 c = (i32)lane; c < nchunks; c += 32)\n";
+    src += "            gdv_cp_async16(dst + 16 * c, src - mis + 16 * c);\n";
+    src += "        }\n";
+    src += "      }\n";
+  }
+  src += "      gdv_cp_async_commit();\n";
+  src += "    };\n";
+  src += "    u32 par = 0u;\n";
+  src += "    if (wbase + " + s32R + " <= A.n) issue(wbase, 0u);\n";
+  src += "    #pragma unroll 1\n";
+  src += "    for (int g = 0; g < 32; g += " + sR + ") {\n";
+  src += "      const i64 base = wbase + 32 * g;\n";
+  src += "      if (base >= A.n) break;\n";
+  for (size_t j = 0; j < slots.size(); ++j)
+    if (HasByteRun(slots[j]))
+      src += "      u8* const stage" + std::to_string(j) + " = stage" + std::to_string(j) +
+             "_0 + (size_t)par * " + std::to_string(stage_bytes) + "u;\n";
+  src += "      if (base + " + s32R + " <= A.n) {\n";
+  src += "        if (g + " + sR + " < 32 && base + " + std::to_string(64 * R) + " <= A.n) {\n";
+  src += "          issue(base + " + s32R + ", par ^ 1u);\n";
+  src += "          gdv_cp_async_wait<1>();\n";
+  src += "        } else {\n";
+  src += "          gdv_cp_async_wait<0>();\n";
+  src += "        }\n";
+  src += "        __syncwarp();\n";
+  src += "        par ^= 1u;\n";
+  EmitGroup(slots, spec, false, R, kFast, body, step_tail, &src, 4, stage_bytes, std::string(), coop, true);
+  src += "      } else {\n";
+  EmitGroup(slots, spec, false, R, kPred, body, step_tail, &src, 4, 0, std::string(), coop);
+  src += "      }\n";
+  src += "    }\n";
+  src += "    mymask[0] = cur;\n";
+}
+
+// Filter: every warp owns 1024 consecutive rows per chunk (32 steps of 32 rows).  Step k's
+// keep-mask is one ballot word, parked in lane k, so a chunk costs one register per thread
+// regardless of its size; loads are issued R steps at a time for memory-level parallelism.
+// Large tiles keep the number of look-back descriptors per launch small, which is what bounds
+// ordered compaction at HBM bandwidth (DESIGN.md "Filter kernel").
+Status GenerateFilter(const Schema& schema, const std::vector<ExpressionPtr>& exprs, const KernelSpec& spec,
+                      GeneratedKernel* out) {
+  std::vector<ColumnSlot> slots;
+  BodyGen gen = SpecBodyGen(schema, &slots, spec);
+  // Per-row body (uses f<j>[k] / k<j>[k]); generated first so we know the slots.
+  std::string body;
+  std::vector<Val> results;
+  for (const auto& e : exprs) results.push_back(gen.GenTruth(*e->root(), &body, 4));
+  if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
+  if (spec.nullable && !gen.uses_ctx() && exprs.size() == 1) MarkHoisted(gen, *exprs[0]->root(), &slots);
+  // Fixed-width Filter: gated loads (EmitGatedGroup) wherever PlanGate finds a plan.  gate_seg[s] ANDs
+  // stage s's conjuncts into alive[k]; the segments come from a BodyGen of their own (over the same
+  // slots), whose globals replace those of `body`, which a gated kernel does not emit.
+  GatePlan gate;
+  std::vector<std::string> gate_seg;
+  std::vector<ColumnSlot> gate_slots = slots;
+  BodyGen sgen = SpecBodyGen(schema, &gate_slots, spec);
+  if (spec.filter_gating == 0 && exprs.size() == 1 && PlanGate(schema, *exprs[0]->root(), slots, &gate)) {
+    for (const auto& cj : gate.conjuncts) {
+      std::string seg, all;
+      for (const Node* c : cj) all += " && (" + sgen.GenTruth(*c, &seg, 6).v + ")";
+      gate_seg.push_back(seg + "            alive[k] = alive[k]" + all + ";\n");
+    }
+  }
+  const bool gated = !gate_seg.empty();
+  DescribeKernel(spec, slots, 0, out);
+  int R = spec.rows_per_thread > 0 ? spec.rows_per_thread : PickRowsPerThread(out->in_bytes_per_row, 0, spec.kind);
+  if (R > 32) R = 32;
+  // the filter walks 32 steps per warp in groups of R: R must divide 32
+  int p = 1;
+  while (p * 2 <= R) p *= 2;
+  R = p;
+  // Filters copy the string bytes of the NEXT group into a second stage with cp.async while the
+  // current group is scanned (per-warp double buffering): the copy costs no registers and its
+  // latency is hidden behind the scan instead of behind other warps.
+  int BT = 0;
+  StringStages st;
+  const Status fit = FitStages(spec, gen, slots, 2, &R, &BT, &st);
+  if (!fit.ok()) return fit;
+  const int n_varlen = st.columns;
+  // 1024-row chunks every warp walks per tile (Configuration.stages; 1 unless asked)
+  const int W = n_varlen != 0 ? 1
+                : (spec.stages == 1 || spec.stages == 2 || spec.stages == 4 || spec.stages == 8) ? spec.stages
+                : (spec.large_batch ? 4 : 1);
+  out->rows_per_thread = R;
+  out->block_threads = BT;
+
+  std::string header = HeaderLines("one fused kernel per Filter", spec, exprs);
+  if (gated) header += "// gated loads: " + std::to_string(gate.stages()) + " stages\n";
+  // Fixed-width filters are bandwidth-bound and want every warp slot of the SM: ask for
+  // 2048 / BT resident CTAs, which caps the kernel at 32 registers per thread (what it needs).
+  std::string bounds = std::to_string(BT);
+  bool light = n_varlen == 0 && BT >= 256 && 2048 % BT == 0 && !gen.uses_ctx() && body.size() < 6000;
+  for (const auto& sl : slots)  // 128-bit math and string functions over dictionary views want registers
+    light = light && !sl.type.is_decimal() && !sl.type.is_dict() && !sl.type.is_view();
+  if (light && W > 1 && gated) {
+    // the stage chain keeps more values live than the ungated group: hold the 48 warps per SM that
+    // the ungated kernel reaches at W > 1 (40 registers)
+    bounds += ", " + std::to_string(1536 / BT);
+    light = false;
+  }
+  if (W > 1) light = false;  // W chunks keep 2 W more registers
+  if (light) bounds += ", " + std::to_string(2048 / BT);
+  std::string src = EmitKernelFrame(spec, false, *out, gated ? sgen : gen, header, bounds);
+  if (st.stage_bytes > 0)
+    src += EmitStageDecls(slots, gen.coop_segs(), st, "u8* const ", "_0", ";  // [0] hits, [1] candidates\n");
+
+  const std::string IDX = SelCType(spec.selection_mode);
+  const int NW = BT / 32;
+  const int WT = NW * 1024 * W;
+  src += "  __shared__ u32 s_wcount[" + std::to_string(NW) + "];\n";
+  src += "  __shared__ i64 s_tile;\n";
+  src += "  __shared__ u64 s_excl;\n";
+  src += "  const i64 n_tiles = (A.n + " + std::to_string(WT - 1) + ") / " + std::to_string(WT) + ";\n";
+  src += "  " + IDX + "* out_idx = reinterpret_cast<" + IDX + "*>(A.out_idx);\n";
+  src += "  const u32 lt = gdv_lanemask_lt();\n";
+  src += "  while (true) {\n";
+  src += "    if (threadIdx.x == 0) s_tile = (i64)atomicAdd(A.ticket, 1ull);\n";
+  src += "    __syncthreads();\n";
+  src += "    const i64 tile = s_tile;\n";
+  src += "    if (tile >= n_tiles) break;\n";
+  src += "    const i64 wbase0 = tile * " + std::to_string(WT) + " + (i64)wid * " + std::to_string(1024 * W) + ";\n";
+  src += "    u32 mymask[" + std::to_string(W) + "];\n";
+  const std::string step_tail =
+      "          { const u32 m = __ballot_sync(GDV_FULL, in && (" + results[0].ok + ") && (" +
+      results[0].v + ")); if (lane == (u32)(g + k)) cur = m; }\n";
+  if (n_varlen == 0)
+    EmitChunkLoop(slots, spec, R, W, body, step_tail, gen.coop_segs(), gate, gate_seg, &src);
+  else
+    EmitPrefetchLoop(slots, spec, R, st.stage_bytes, body, step_tail, gen.coop_segs(), &src);
+  EmitFilterEpilogue(slots, spec, NW, W, IDX, &src);
+  src += "  }\n";
+  src += "}\n";
+
+  out->source = std::move(src);
+  out->uses_ctx = gen.uses_ctx();
+  out->dynamic_smem = st.dynamic_smem(BT);
+  out->tile_rows = static_cast<int64_t>(NW) * 1024 * W;
+  out->cta_tile_rows = static_cast<int64_t>(BT) * R;
+  out->view_shortcuts = gen.view_shortcuts();
+  out->gated_stages = gated ? gate.stages() : 0;
+  return Status::OK();
+}
+
+// ---- Projector ----------------------------------------------------------------------------------
+// Per-step tail of a projector group: the stores (`fast`: every row of the group is in range) and the
+// validity / boolean-data ballots into lane k's words.
+std::string ProjectStepTail(const std::vector<ExpressionPtr>& exprs, const std::vector<Val>& results, bool fast) {
+  std::string t5;
+  for (size_t o = 0; o < exprs.size(); ++o) {
+    const DataType& t = exprs[o]->result().type;
+    const std::string O = std::to_string(o);
+    if (t.is_bool()) {
+      t5 += "        { const u32 m = __ballot_sync(GDV_FULL, in && (" + results[o].v +
+            ")); if (lane == (u32)k) dw" + O + " = m; }\n";
+    } else if (fast) {
+      t5 += "        gdv_stp(out" + O + " + s, (" + std::string(t.ctype()) + ")(" + results[o].v +
+            "));\n";
+    } else {
+      t5 += "        if (in) gdv_stp(out" + O + " + s, (" + std::string(t.ctype()) + ")(" +
+            results[o].v + "));\n";
+    }
+    t5 += "        { const u32 m = __ballot_sync(GDV_FULL, in && (" + results[o].ok +
+          ")); if (lane == (u32)k) vw" + O + " = m; }\n";
+  }
+  return t5;
+}
+
+// A warp tile's output words, one per 32 rows and held by lane k for step k: validity vw<o> and,
+// for a boolean output, its bit-packed data dw<o>.
+std::string EmitOutWordDecls(const std::vector<ExpressionPtr>& exprs) {
+  std::string o;
+  for (size_t i = 0; i < exprs.size(); ++i) {
+    o += "    u32 vw" + std::to_string(i) + " = 0u;\n";
+    if (exprs[i]->result().type.is_bool()) o += "    u32 dw" + std::to_string(i) + " = 0u;\n";
+  }
+  return o;
+}
+
+// Their write-back: lanes k < R (and `guard`) store word k of the warp tile that starts at `base`.
+std::string EmitOutWordStores(const std::vector<ExpressionPtr>& exprs, int R, const std::string& guard) {
+  std::string o = "    if (lane < " + std::to_string(R) + "u" + guard + ") {\n";
+  o += "      const i64 w = (base >> 5) + (i64)lane;\n";
+  for (size_t i = 0; i < exprs.size(); ++i) {
+    const std::string O = std::to_string(i);
+    o += "      if (A.out_vld[" + O + "] != nullptr) A.out_vld[" + O + "][w] = vw" + O + ";\n";
+    if (exprs[i]->result().type.is_bool()) o += "      reinterpret_cast<u32*>(A.out_val[" + O + "])[w] = dw" + O + ";\n";
+  }
+  return o + "    }\n";
+}
+
+// TMA loader (fixed-width inputs, no selection vector): each CTA tile (BT * R rows) of every input
+// column is copied into a shared-memory stage by one cp.async.bulk; S stages per CTA keep (S - 1)
+// tiles in flight per CTA while one computes.  Emits the loop over the staged tiles of the kernel
+// `out` describes and sets its staged / stages / dynamic_smem; false, with nothing emitted, when two
+// stages do not fit.
+bool EmitStagedTiles(const KernelSpec& spec, const std::vector<ExpressionPtr>& exprs, const std::string& body,
+                     const std::vector<Val>& results, const std::vector<CoopSeg>& coop, std::string* o,
+                     GeneratedKernel* out) {
+  const std::vector<ColumnSlot>& slots = out->inputs;
+  const int R = out->rows_per_thread, BT = out->block_threads;
+  std::vector<int> val_off(slots.size(), 0), vld_off(slots.size(), 0);
+  int stage_total = 0, val_tx = 0, S = 0;
+  const int vld_copy = BT * R / 8 + 32;
+  int off = 0;
+  for (size_t j = 0; j < slots.size(); ++j) {
+    val_off[j] = off;
+    off += BT * R * slots[j].type.width() + 16;
+    val_tx += BT * R * slots[j].type.width() + 16;
+  }
+  if (spec.nullable)
+    for (size_t j = 0; j < slots.size(); ++j) {
+      vld_off[j] = off;
+      off += vld_copy;
+    }
+  stage_total = (off + 127) / 128 * 128;
+  S = spec.stages > 0 ? spec.stages : 4;
+  while (S > 2 && S * stage_total > 220 * 1024) --S;
+  if (S < 2 || S * stage_total > 220 * 1024) return false;
+  out->dynamic_smem = S * stage_total;
+  out->staged = true;
+  out->stages = S;
+
+  std::string& src = *o;
+  const int T = BT * R;  // rows per CTA tile
+  const std::string sS = std::to_string(S), sT = std::to_string(T), s32R = std::to_string(32 * R);
+  src += "  extern __shared__ uint4 gdv_smem[];\n";
+  src += "  __shared__ u64 gdv_full[" + sS + "];\n";
+  src += "  u8* const stage0 = reinterpret_cast<u8*>(gdv_smem);\n";
+  std::string tx = std::to_string(val_tx) + "u";
+  for (size_t j = 0; j < slots.size(); ++j) {
+    const std::string J = std::to_string(j);
+    src += "  const u32 mis" + J + " = (u32)((unsigned long long)in_val" + J + " & 15ull);\n";
+    if (spec.nullable) {
+      src += "  const u32 vmis" + J + " = (u32)((unsigned long long)in_vld" + J + " & 15ull);\n";
+      tx += " + (in_hv" + J + " ? " + std::to_string(vld_copy) + "u : 0u)";
+    }
+  }
+  src += "  const u32 tx_bytes = " + tx + ";\n";
+  src += "  const u64 pol = gdv_policy_evict_first();\n";
+  // a bulk copy may read up to 32 bytes past its tile: the last 256 rows are never staged
+  src += "  const i64 n_st = A.n > 256 ? (A.n - 256) / " + sT + " : 0;\n";
+  src += "  if (threadIdx.x == 0) {\n";
+  src += "    for (u32 s = 0; s < " + sS + "u; ++s) gdv_mbar_init(&gdv_full[s], 1u);\n";
+  src += "    gdv_fence_mbar_init();\n";
+  src += "  }\n";
+  src += "  __syncthreads();\n";
+  src += "  auto issue = [&](i64 t, u32 s) {\n";
+  src += "    u8* sb = stage0 + (size_t)s * " + std::to_string(stage_total) + "u;\n";
+  src += "    gdv_mbar_expect_tx(&gdv_full[s], tx_bytes);\n";
+  for (size_t j = 0; j < slots.size(); ++j) {
+    const std::string J = std::to_string(j);
+    const int w = slots[j].type.width();
+    src += "    gdv_bulk_g2s(sb + " + std::to_string(val_off[j]) + ", reinterpret_cast<const u8*>(in_val" +
+           J + ") - mis" + J + " + t * " + std::to_string(static_cast<long long>(T) * w) + "ll, " +
+           std::to_string(T * w + 16) + "u, &gdv_full[s], pol);\n";
+    if (spec.nullable)
+      src += "    if (in_hv" + J + ") gdv_bulk_g2s(sb + " + std::to_string(vld_off[j]) +
+             ", reinterpret_cast<const u8*>(in_vld" + J + ") - vmis" + J + " + t * " +
+             std::to_string(T / 8) + "ll, " + std::to_string(vld_copy) + "u, &gdv_full[s], pol);\n";
+  }
+  src += "  };\n";
+  src += "  if (threadIdx.x == 0) {\n";
+  src += "    for (u32 s = 0; s < " + sS + "u; ++s) {\n";
+  src += "      const i64 t = (i64)blockIdx.x + (i64)s * gridDim.x;\n";
+  src += "      if (t < n_st) issue(t, s);\n";
+  src += "    }\n";
+  src += "  }\n";
+  src += "  u32 it = 0u;\n";
+  src += "  for (i64 t = blockIdx.x; t < n_st; t += gridDim.x, ++it) {\n";
+  src += "    const u32 s = it % " + sS + "u;\n";
+  src += "    const u32 par = (it / " + sS + "u) & 1u;\n";
+  src += "    const u8* sb = stage0 + (size_t)s * " + std::to_string(stage_total) + "u;\n";
+  src += "    const i64 base = t * " + sT + " + (i64)wid * " + s32R + ";\n";
+  for (size_t j = 0; j < slots.size(); ++j) {
+    const std::string J = std::to_string(j);
+    const std::string ct = slots[j].type.ctype();
+    src += "    const " + ct + "* sp" + J + " = reinterpret_cast<const " + ct + "*>(sb + " +
+           std::to_string(val_off[j]) + " + mis" + J + ") + wid * " + s32R + "u + lane;\n";
+    if (spec.nullable)
+      src += "    const u32* sv" + J + " = reinterpret_cast<const u32*>(sb + " +
+             std::to_string(vld_off[j]) + " + vmis" + J + ");\n";
+  }
+  src += EmitOutWordDecls(exprs);
+  src += "    gdv_mbar_wait(&gdv_full[s], par);\n";
+  src += "    {\n";
+  std::string after;
+  after += "      __syncthreads();  // every thread holds its rows: the stage can be refilled\n";
+  after += "      if (threadIdx.x == 0) {\n";
+  after += "        const i64 tn = t + (i64)" + sS + " * gridDim.x;\n";
+  after += "        if (tn < n_st) issue(tn, s);\n";
+  after += "      }\n";
+  EmitGroup(slots, spec, false, R, kStaged, body, ProjectStepTail(exprs, results, true), &src, 3, 0, after, coop);
+  src += "    }\n";
+  src += EmitOutWordStores(exprs, R, "");
+  src += "  }\n";
+  return true;
+}
+
+// Direct loads: warp tiles of 32 R rows, from warp tile `wt_first` on (the rows after the staged tiles).
+void EmitDirectTiles(const KernelSpec& spec, bool has_sel, const std::vector<ExpressionPtr>& exprs,
+                     const std::string& body, const std::vector<Val>& results, const std::vector<CoopSeg>& coop,
+                     int stage_bytes, const std::string& wt_first, const GeneratedKernel& out, std::string* o) {
+  std::string& src = *o;
+  const std::vector<ColumnSlot>& slots = out.inputs;
+  const int R = out.rows_per_thread, NWP = out.block_threads / 32;
+  const std::string s32R = std::to_string(32 * R);
+  src += "  const i64 n_wtiles = (A.n + " + std::to_string(32 * R - 1) + ") / " + s32R + ";\n";
+  src += "  const i64 wstride = (i64)gridDim.x * " + std::to_string(NWP) + ";\n";
+  src += "  for (i64 wt = " + wt_first + " + (i64)blockIdx.x * " + std::to_string(NWP) +
+         " + wid; wt < n_wtiles; wt += wstride) {\n";
+  src += "    const i64 base = wt * " + s32R + ";\n";
+  src += EmitOutWordDecls(exprs);
+  if (!has_sel) {
+    src += "    if (base + " + s32R + " <= A.n) {\n";
+    EmitGroup(slots, spec, false, R, kFast, body, ProjectStepTail(exprs, results, true), &src, 3, stage_bytes, std::string(), coop);
+    src += "    } else {\n";
+    EmitGroup(slots, spec, false, R, kPred, body, ProjectStepTail(exprs, results, false), &src, 3, 0, std::string(), coop);
+    src += "    }\n";
+  } else {
+    src += "    {\n";
+    EmitGroup(slots, spec, true, R, kPred, body, ProjectStepTail(exprs, results, false), &src, 3, 0, std::string(), coop);
+    src += "    }\n";
+  }
+  src += EmitOutWordStores(exprs, R, " && base + 32 * (i64)lane < A.n");
+  src += "  }\n";
+}
+
+Status GenerateProjector(const Schema& schema, const std::vector<ExpressionPtr>& exprs, const KernelSpec& spec,
+                         GeneratedKernel* out) {
+  std::vector<ColumnSlot> slots;
+  BodyGen gen = SpecBodyGen(schema, &slots, spec);
+  // Per-row body (uses f<j>[k] / k<j>[k]); generated first so we know the slots.
+  std::string body;
+  std::vector<Val> results;
+  for (const auto& e : exprs) {
+    if (e->result().type.is_varlen())
+      return Status::Make(GDV_NOT_IMPLEMENTED,
+                          "variable-length projection outputs are handled by the two-pass "
+                          "string projector, not by GenerateKernel");
+    results.push_back(gen.Gen(*e->root(), &body, 4));
+  }
+  if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
+  DescribeKernel(spec, slots, static_cast<int>(exprs.size()), out);
+  for (const auto& e : exprs) {
+    out->outputs.push_back(e->result().type);
+    out->out_bytes_per_row += std::max(e->result().type.width(), 1);
+  }
+  // The TMA loader is the default for wide-row projectors (the Q1 projector, 166 B/row): bulk copies
+  // keep a whole tile per column in flight without spending registers on it, where the direct path
+  // runs out of registers before it has enough loads in flight.
+  bool want_staged = spec.selection_mode == GDV_SEL_NONE && spec.loader != 1 && !slots.empty() &&
+                     (spec.loader == 2 || out->in_bytes_per_row >= 48);
+  for (const auto& sl : slots)
+    if (sl.type.is_varlen() || sl.type.is_bool()) want_staged = false;
+  int R = spec.rows_per_thread > 0
+              ? spec.rows_per_thread
+              : (want_staged ? 2 : PickRowsPerThread(out->in_bytes_per_row, out->out_bytes_per_row, spec.kind));
+  if (R > 32) R = 32;
+  int BT = 0;
+  StringStages st;
+  const Status fit = FitStages(spec, gen, slots, 1, &R, &BT, &st);
+  if (!fit.ok()) return fit;
+  out->rows_per_thread = R;
+  out->block_threads = BT;
+  out->dynamic_smem = st.dynamic_smem(BT);
+  const bool has_sel = spec.selection_mode != GDV_SEL_NONE;
+
+  std::string src = EmitKernelFrame(spec, has_sel, *out, gen, HeaderLines("one fused kernel per Projector", spec, exprs),
+                                    std::to_string(BT));
+  if (st.stage_bytes > 0) src += EmitStageDecls(slots, gen.coop_segs(), st, "u8* const ", "", ";  // [0] hits, [1] candidates\n");
+  for (size_t o = 0; o < exprs.size(); ++o) {
+    const DataType& t = exprs[o]->result().type;
+    const std::string O = std::to_string(o);
+    if (!t.is_bool())
+      src += "  " + std::string(t.ctype()) + "* out" + O + " = reinterpret_cast<" + t.ctype() +
+             "*>(A.out_val[" + O + "]);\n";
+  }
+  std::string wt_first = "0";
+  if (want_staged && (BT * R) % 128 == 0 && EmitStagedTiles(spec, exprs, body, results, gen.coop_segs(), &src, out))
+    wt_first = "n_st * " + std::to_string(BT / 32);  // rows after the staged tiles take the direct path
+  EmitDirectTiles(spec, has_sel, exprs, body, results, gen.coop_segs(), st.stage_bytes, wt_first, *out, &src);
+  src += "}\n";
+  if (has_sel) ApplyDeviceCount(&src);
+
+  out->source = std::move(src);
+  out->uses_ctx = gen.uses_ctx();
+  out->cta_tile_rows = static_cast<int64_t>(BT) * R;
   out->view_shortcuts = gen.view_shortcuts();
   return Status::OK();
 }
@@ -2809,111 +3329,51 @@ namespace {
 //   ilike(s, 'pattern') -> like(lower(s), 'lower-cased pattern')   (ASCII case folding)
 // Returns the node itself when nothing below it changes.
 NodePtr RewriteAliases(const NodePtr& node) {
-  switch (node->kind()) {
-    case NodeKind::kFunction: {
-      const auto& fn = static_cast<const FunctionNode&>(*node);
-      NodeVector kids;
-      bool changed = false;
-      for (const auto& c : fn.children()) {
-        kids.push_back(RewriteAliases(c));
-        changed = changed || kids.back() != c;
+  NodeVector kids;
+  for (const auto& c : Children(*node)) kids.push_back(RewriteAliases(c));
+  if (node->kind() == NodeKind::kFunction) {
+    const auto& fn = static_cast<const FunctionNode&>(*node);
+    if (fn.name() == "ilike" && kids.size() == 2 && kids[1]->kind() == NodeKind::kLiteral) {
+      const auto& pat = static_cast<const LiteralNode&>(*kids[1]);
+      std::string low = pat.bytes();
+      for (auto& ch : low)
+        if (ch >= 'A' && ch <= 'Z') ch = static_cast<char>(ch + 32);
+      NodePtr text = std::make_shared<FunctionNode>("lower", NodeVector{kids[0]}, utf8());
+      NodePtr lit = std::make_shared<LiteralNode>(utf8(), low.data(), static_cast<int64_t>(low.size()),
+                                                  pat.is_null());
+      return std::make_shared<FunctionNode>("like", NodeVector{text, lit}, boolean());
+    }
+    // A concat result is a rope that only projection / concat / if-else can read.  Two consumers
+    // distribute over its pieces instead: the ASCII case maps, and the length functions.
+    if (kids.size() == 1 && kids[0]->kind() == NodeKind::kFunction) {
+      const auto& inner = static_cast<const FunctionNode&>(*kids[0]);
+      const bool is_concat = inner.name() == "concat" || inner.name() == "concatOperator";
+      if (is_concat && (fn.name() == "upper" || fn.name() == "lower")) {
+        NodeVector parts;
+        for (const auto& c : inner.children())
+          parts.push_back(RewriteAliases(std::make_shared<FunctionNode>(fn.name(), NodeVector{c}, c->return_type())));
+        return std::make_shared<FunctionNode>(inner.name(), std::move(parts), inner.return_type());
       }
-      if (fn.name() == "ilike" && kids.size() == 2 && kids[1]->kind() == NodeKind::kLiteral) {
-        const auto& pat = static_cast<const LiteralNode&>(*kids[1]);
-        std::string low = pat.bytes();
-        for (auto& ch : low)
-          if (ch >= 'A' && ch <= 'Z') ch = static_cast<char>(ch + 32);
-        NodePtr text = std::make_shared<FunctionNode>("lower", NodeVector{kids[0]}, utf8());
-        NodePtr lit = std::make_shared<LiteralNode>(utf8(), low.data(), static_cast<int64_t>(low.size()),
-                                                    pat.is_null());
-        return std::make_shared<FunctionNode>("like", NodeVector{text, lit}, boolean());
-      }
-      // A concat result is a rope that only projection / concat / if-else can read.  Two consumers
-      // distribute over its pieces instead: the ASCII case maps, and the length functions.
-      if (kids.size() == 1 && kids[0]->kind() == NodeKind::kFunction) {
-        const auto& inner = static_cast<const FunctionNode&>(*kids[0]);
-        const bool is_concat = inner.name() == "concat" || inner.name() == "concatOperator";
-        if (is_concat && (fn.name() == "upper" || fn.name() == "lower")) {
-          NodeVector parts;
-          for (const auto& c : inner.children())
-            parts.push_back(RewriteAliases(std::make_shared<FunctionNode>(fn.name(), NodeVector{c}, c->return_type())));
-          return std::make_shared<FunctionNode>(inner.name(), std::move(parts), inner.return_type());
+      const bool is_len = fn.name() == "char_length" || fn.name() == "length" || fn.name() == "lengthUtf8" ||
+                          fn.name() == "octet_length" || fn.name() == "bit_length";
+      if (is_concat && is_len && !inner.children().empty()) {
+        // concat counts a NULL argument as the empty string; concatOperator is NULL if any argument is
+        NodePtr sum;
+        const int32_t zero = 0;
+        for (const auto& c : inner.children()) {
+          NodePtr len = RewriteAliases(std::make_shared<FunctionNode>(fn.name(), NodeVector{c}, fn.return_type()));
+          if (inner.name() == "concat")
+            len = std::make_shared<FunctionNode>(
+                "nvl", NodeVector{len, std::make_shared<LiteralNode>(fn.return_type(), &zero, 4, false)}, fn.return_type());
+          sum = sum == nullptr ? len : std::make_shared<FunctionNode>("add", NodeVector{sum, len}, fn.return_type());
         }
-        const bool is_len = fn.name() == "char_length" || fn.name() == "length" || fn.name() == "lengthUtf8" ||
-                            fn.name() == "octet_length" || fn.name() == "bit_length";
-        if (is_concat && is_len && !inner.children().empty()) {
-          // concat counts a NULL argument as the empty string; concatOperator is NULL if any argument is
-          NodePtr sum;
-          const int32_t zero = 0;
-          for (const auto& c : inner.children()) {
-            NodePtr len = RewriteAliases(std::make_shared<FunctionNode>(fn.name(), NodeVector{c}, fn.return_type()));
-            if (inner.name() == "concat")
-              len = std::make_shared<FunctionNode>(
-                  "nvl", NodeVector{len, std::make_shared<LiteralNode>(fn.return_type(), &zero, 4, false)}, fn.return_type());
-            sum = sum == nullptr ? len : std::make_shared<FunctionNode>("add", NodeVector{sum, len}, fn.return_type());
-          }
-          return sum;
-        }
+        return sum;
       }
-      if (!changed) return node;
-      return std::make_shared<FunctionNode>(fn.name(), std::move(kids), fn.return_type());
     }
-    case NodeKind::kIf: {
-      const auto& n = static_cast<const IfNode&>(*node);
-      NodePtr c = RewriteAliases(n.condition()), t = RewriteAliases(n.then_node()),
-              e = RewriteAliases(n.else_node());
-      if (c == n.condition() && t == n.then_node() && e == n.else_node()) return node;
-      return std::make_shared<IfNode>(c, t, e, n.return_type());
-    }
-    case NodeKind::kBoolean: {
-      const auto& n = static_cast<const BooleanNode&>(*node);
-      NodeVector kids;
-      bool changed = false;
-      for (const auto& c : n.children()) {
-        kids.push_back(RewriteAliases(c));
-        changed = changed || kids.back() != c;
-      }
-      if (!changed) return node;
-      return std::make_shared<BooleanNode>(n.op(), std::move(kids));
-    }
-    case NodeKind::kIn: {
-      const auto& n = static_cast<const InNode&>(*node);
-      NodePtr c = RewriteAliases(n.child());
-      if (c == n.child()) return node;
-      return std::make_shared<InNode>(c, n.value_type(), n.ints(), n.strs());
-    }
-    default: return node;
   }
+  return WithChildren(node, std::move(kids));
 }
 
-Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>& exprs,
-                          const KernelSpec& spec, GeneratedKernel* out);
-
-}  // namespace
-
-namespace {
-void CollectColumns(const Schema& schema, const Node& node, std::vector<int>* cols) {
-  switch (node.kind()) {
-    case NodeKind::kField: {
-      const int i = schema.index_of(static_cast<const FieldNode&>(node).name());
-      if (std::find(cols->begin(), cols->end(), i) == cols->end()) cols->push_back(i);
-      return;
-    }
-    case NodeKind::kLiteral: return;
-    case NodeKind::kFunction:
-      for (const auto& c : static_cast<const FunctionNode&>(node).children()) CollectColumns(schema, *c, cols);
-      return;
-    case NodeKind::kIf: {
-      const auto& n = static_cast<const IfNode&>(node);
-      for (const NodePtr* c : {&n.condition(), &n.then_node(), &n.else_node()}) CollectColumns(schema, **c, cols);
-      return;
-    }
-    case NodeKind::kBoolean:
-      for (const auto& c : static_cast<const BooleanNode&>(node).children()) CollectColumns(schema, *c, cols);
-      return;
-    case NodeKind::kIn: CollectColumns(schema, *static_cast<const InNode&>(node).child(), cols); return;
-  }
-}
 }  // namespace
 
 int DictionaryFirstColumn(const Schema& schema, const Node& cond) {
@@ -2929,56 +3389,17 @@ int DictionaryFirstColumn(const Schema& schema, const Node& cond) {
 }
 
 NodePtr WithValueTypes(const NodePtr& node) {
-  switch (node->kind()) {
-    case NodeKind::kField: {
-      const auto& f = static_cast<const FieldNode&>(*node);
-      if (!f.return_type().is_dict()) return node;
-      return std::make_shared<FieldNode>(f.name(), f.return_type().value_type());
-    }
-    case NodeKind::kLiteral: return node;
-    case NodeKind::kFunction: {
-      const auto& fn = static_cast<const FunctionNode&>(*node);
-      NodeVector kids;
-      for (const auto& c : fn.children()) kids.push_back(WithValueTypes(c));
-      return std::make_shared<FunctionNode>(fn.name(), std::move(kids), fn.return_type());
-    }
-    case NodeKind::kIf: {
-      const auto& n = static_cast<const IfNode&>(*node);
-      return std::make_shared<IfNode>(WithValueTypes(n.condition()), WithValueTypes(n.then_node()),
-                                      WithValueTypes(n.else_node()), n.return_type());
-    }
-    case NodeKind::kBoolean: {
-      const auto& n = static_cast<const BooleanNode&>(*node);
-      NodeVector kids;
-      for (const auto& c : n.children()) kids.push_back(WithValueTypes(c));
-      return std::make_shared<BooleanNode>(n.op(), std::move(kids));
-    }
-    case NodeKind::kIn: {
-      const auto& n = static_cast<const InNode&>(*node);
-      return std::make_shared<InNode>(WithValueTypes(n.child()), n.value_type(), n.ints(), n.strs());
-    }
-  }
-  return node;
+  if (node->kind() == NodeKind::kField && node->return_type().is_dict())
+    return std::make_shared<FieldNode>(static_cast<const FieldNode&>(*node).name(), node->return_type().value_type());
+  NodeVector kids;
+  for (const auto& c : Children(*node)) kids.push_back(WithValueTypes(c));
+  return WithChildren(node, std::move(kids));
 }
 
-static bool ReadsDictionary(const Node& node) {
-  switch (node.kind()) {
-    case NodeKind::kField: return node.return_type().is_dict() || node.return_type().is_view();
-    case NodeKind::kLiteral: return false;
-    case NodeKind::kFunction:
-      for (const auto& c : static_cast<const FunctionNode&>(node).children())
-        if (ReadsDictionary(*c)) return true;
-      return false;
-    case NodeKind::kIf: {
-      const auto& n = static_cast<const IfNode&>(node);
-      return ReadsDictionary(*n.condition()) || ReadsDictionary(*n.then_node()) || ReadsDictionary(*n.else_node());
-    }
-    case NodeKind::kBoolean:
-      for (const auto& c : static_cast<const BooleanNode&>(node).children())
-        if (ReadsDictionary(*c)) return true;
-      return false;
-    case NodeKind::kIn: return ReadsDictionary(*static_cast<const InNode&>(node).child());
-  }
+static bool ReadsDictionaryOrView(const Node& node) {
+  if (node.kind() == NodeKind::kField) return node.return_type().is_dict() || node.return_type().is_view();
+  for (const auto& c : Children(node))
+    if (ReadsDictionaryOrView(*c)) return true;
   return false;
 }
 
@@ -2991,543 +3412,16 @@ Status GenerateKernel(const Schema& schema, const std::vector<ExpressionPtr>& ex
     lowered.push_back(r == e->root() ? e : std::make_shared<Expression>(r, e->result()));
     // a dictionary row is null when its entry is, or when its index is out of range, and a view row
     // when its view is invalid: such kernels always keep the validity plumbing
-    if (ReadsDictionary(*r)) s.nullable = true;
+    if (ReadsDictionaryOrView(*r)) s.nullable = true;
   }
-  return GenerateKernelImpl(schema, lowered, s, out);
-}
-
-namespace {
-
-Status GenerateKernelImpl(const Schema& schema, const std::vector<ExpressionPtr>& exprs,
-                          const KernelSpec& spec, GeneratedKernel* out) {
-  if (spec.kind == KernelKind::kStringSize || spec.kind == KernelKind::kStringWrite) {
-    if (exprs.size() != 1 || !exprs[0]->result().type.is_varlen())
+  if (s.kind == KernelKind::kStringSize || s.kind == KernelKind::kStringWrite) {
+    if (lowered.size() != 1 || !lowered[0]->result().type.is_varlen())
       return Status::Make(GDV_INVALID, "a string kernel takes exactly one utf8/binary expression");
-    return GenerateStringKernel(schema, exprs[0], spec, out);
+    return GenerateStringKernel(schema, lowered[0], s, out);
   }
-  // Key-driven string filter (default wherever it applies; string_scan bit 2 keeps the row-driven
-  // kernel): driven by the occurrences of a literal of the condition in the column's bytes.
-  // Conditions that can raise keep the row-driven kernel so that errors come from the same rows.
-  if (spec.kind == KernelKind::kFilter && (spec.string_scan & 4) == 0 && exprs.size() == 1 &&
-      !BodyGen::CanFail(*exprs[0]->root())) {
-    std::vector<ColumnSlot> kslots;
-    BodyGen kgen(schema, &kslots, spec.nullable, /*coop=*/false);
-    KeyPlan plan;
-    const int kBT = spec.block_threads > 0 ? spec.block_threads : 256;
-    // chunks of 1024 rows per warp and tile: more rows per anchor drain and per tile-end barrier on
-    // big batches (Configuration.stages overrides), one on small ones (enough tiles for 132 SMs)
-    const int kW = (spec.stages == 1 || spec.stages == 2 || spec.stages == 4) ? spec.stages : (spec.large_batch ? 2 : 1);
-    if (kBT % 32 == 0 && kBT <= 1024 && kgen.PlanKey(*exprs[0]->root(), &plan)) {
-      std::string kbody;
-      const Val kres = kgen.GenTruth(*exprs[0]->root(), &kbody, 6);
-      // the anchor drain loads rows one by one from plain columns only
-      if (kgen.error().empty() && !kgen.uses_ctx() && !HasDictionary(kslots) && !HasView(kslots)) {
-        if (spec.nullable) MarkHoisted(kgen, *exprs[0]->root(), &kslots);
-        ArgsLayout KL(static_cast<int>(kslots.size()), 0);
-        std::string src = "// generated by gandiva_b200 kernel fuser; key-driven string Filter";
-        src += spec.nullable ? " (inputs may carry validity bitmaps)\n" : " (no input has nulls)\n";
-        src += "// expr_0: " + CommentSafe(exprs[0]->ToString()) + "\n";
-        src += "// key: '" + CommentSafe(plan.key) + "' in column slot " + std::to_string(plan.slot) +
-               ", case map " + std::to_string(plan.xf) + "\n";
-        src += "#include \"gdv_device_lib.cuh\"\n";
-        src += EmitArgsStruct(KL);
-        src += kgen.globals();
-        src += EmitKeyFilter(kslots, spec, plan, kbody, kres, kBT, kW, kgen.ScratchDecl(1));
-        int in_bytes = 0;
-        for (const auto& sl : kslots) in_bytes += sl.type.is_varlen() ? 32 : std::max(sl.type.width(), 1);
-        out->source = std::move(src);
-        out->name = spec.name;
-        out->kind = spec.kind;
-        out->rows_per_thread = 1;
-        out->block_threads = kBT;
-        out->selection_mode = spec.selection_mode;
-        out->nullable = spec.nullable;
-        out->inputs = kslots;
-        out->outputs.clear();
-        out->uses_ctx = false;
-        out->in_bytes_per_row = in_bytes;
-        out->out_bytes_per_row = 0;
-        out->args_size = KL.size;
-        out->dynamic_smem = (kBT / 32) * (kKeyAnchorCap + 32 * kW + 4) * 4;
-        out->tile_rows = static_cast<int64_t>(kBT / 32) * 1024 * kW;
-        out->key_driven = true;
-        out->staged = false;
-        out->stages = 0;
-        out->cta_tile_rows = 0;
-        return Status::OK();
-      }
-    }
-  }
-  std::vector<ColumnSlot> slots;
-  BodyGen gen(schema, &slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
-
-  // Per-row body (uses f<j>[k] / k<j>[k]); generated first so we know the slots.
-  std::string body;
-  std::vector<Val> results;
-  for (const auto& e : exprs) {
-    if (spec.kind == KernelKind::kProject && e->result().type.is_varlen())
-      return Status::Make(GDV_NOT_IMPLEMENTED,
-                          "variable-length projection outputs are handled by the two-pass "
-                          "string projector, not by GenerateKernel");
-    results.push_back(spec.kind == KernelKind::kFilter ? gen.GenTruth(*e->root(), &body, 4)
-                                                       : gen.Gen(*e->root(), &body, 4));
-  }
-  if (!gen.error().empty()) return Status::Make(GDV_NOT_IMPLEMENTED, gen.error());
-  if (spec.kind == KernelKind::kFilter && spec.nullable && !gen.uses_ctx() && exprs.size() == 1)
-    MarkHoisted(gen, *exprs[0]->root(), &slots);
-  // Fixed-width Filter: gated loads (EmitGatedGroup) wherever PlanGate finds a plan.  gate_seg[s] ANDs
-  // stage s's conjuncts into alive[k]; the segments come from a BodyGen of their own (over the same
-  // slots), whose globals replace those of `body`, which a gated kernel does not emit.
-  GatePlan gate;
-  std::vector<std::string> gate_seg;
-  std::vector<ColumnSlot> gate_slots = slots;
-  BodyGen sgen(schema, &gate_slots, spec.nullable, (spec.string_scan & 1) == 0, (spec.string_scan & 8) == 0);
-  if (spec.kind == KernelKind::kFilter && spec.filter_gating == 0 && exprs.size() == 1 &&
-      PlanGate(schema, *exprs[0]->root(), slots, &gate)) {
-    for (const auto& cj : gate.conjuncts) {
-      std::string seg, all;
-      for (const Node* c : cj) all += " && (" + sgen.GenTruth(*c, &seg, 6).v + ")";
-      gate_seg.push_back(seg + "            alive[k] = alive[k]" + all + ";\n");
-    }
-  }
-  const bool gated = !gate_seg.empty();
-
-  int in_bytes = 0, out_bytes = 0;
-  int n_varlen = 0;
-  for (const auto& s : slots) {
-    in_bytes += s.type.is_dict() ? DataType(s.type.index).width()  // the index; the dictionary is cached
-                : s.type.is_view()   ? 16                               // the view; out-of-line bytes on demand
-                : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);  // 4 B offset + ~28 B data
-    n_varlen += HasByteRun(s) ? 1 : 0;
-  }
-  for (const auto& e : exprs) out_bytes += std::max(e->result().type.width(), 1);
-  if (spec.kind == KernelKind::kFilter) out_bytes = 0;
-
-  // The TMA loader is the default for wide-row projectors (the Q1 projector, 166 B/row): bulk copies
-  // keep a whole tile per column in flight without spending registers on it.
-  bool want_staged = spec.kind == KernelKind::kProject && spec.selection_mode == GDV_SEL_NONE &&
-                     spec.loader != 1 && !slots.empty() && (spec.loader == 2 || in_bytes >= 48);
-  for (const auto& sl : slots)
-    if (sl.type.is_varlen() || sl.type.is_bool()) want_staged = false;
-  int R = spec.rows_per_thread > 0 ? spec.rows_per_thread
-                                   : (want_staged ? 2 : PickRowsPerThread(in_bytes, out_bytes, spec.kind));
-  if (R > 32) R = 32;
-  if (spec.kind == KernelKind::kFilter) {
-    // the filter walks 32 steps per warp in groups of R: R must divide 32
-    int p = 1;
-    while (p * 2 <= R) p *= 2;
-    R = p;
-  }
-  // String predicates are instruction-bound and stage bytes per warp in shared memory: they run
-  // 512 threads on big batches; everything else runs 256.
-  int BT = spec.block_threads > 0 ? spec.block_threads
-                                  : (spec.kind == KernelKind::kFilter && n_varlen > 0 && spec.large_batch ? 512 : 256);
-  if (BT % 32 != 0 || BT > 1024)
-    return Status::Make(GDV_INVALID, "block_threads must be a multiple of 32 and <= 1024");
-
-  // Filters copy the string bytes of the NEXT group into a second stage with cp.async while the
-  // current group is scanned (per-warp double buffering): the copy costs no registers and its
-  // latency is hidden behind the scan instead of behind other warps.
-  const bool prefetch = spec.kind == KernelKind::kFilter && n_varlen > 0;
-  const int n_stages = prefetch ? 2 : 1;
-  // Many string columns (e.g. a schema extended by materialised ropes, gdv_rope_temps.h): the per-warp stages
-  // of all of them must fit the CTA's shared memory — fewer rows per thread first, then fewer warps per CTA.
-  {
-    const int hit = gen.coop_segs().empty() ? 0 : 8 * kHitCap + 16;
-    auto need = [&](int r, int bt) { return (n_stages * 48 * 32 * r + hit) * (bt / 32) * n_varlen; };
-    const int kMaxStage = 200 * 1024;
-    while (need(R, BT) > kMaxStage && R > 1) R /= 2;
-    while (need(R, BT) > kMaxStage && BT > 64 && spec.block_threads == 0) BT /= 2;
-    if (need(R, BT) > kMaxStage)
-      return Status::Make(GDV_NOT_IMPLEMENTED, "too many utf8/binary columns for one kernel (" + std::to_string(n_varlen) + ")");
-  }
-  // shared-memory stage for string bytes: 48 B per row of a group, per warp and string column
-  const int stage_bytes = n_varlen > 0 ? 48 * 32 * R : 0;
-  // fixed-width filters: 1024-row chunks every warp walks per tile (Configuration.stages; 1 unless asked)
-  const int W = (spec.kind != KernelKind::kFilter || n_varlen != 0) ? 1
-                : (spec.stages == 1 || spec.stages == 2 || spec.stages == 4 || spec.stages == 8) ? spec.stages
-                : (spec.large_batch ? 4 : 1);
-  // per warp and string column: [stage bytes x stages][hit list + counters of the cooperative scan]
-  const std::vector<CoopSeg>& coop = gen.coop_segs();
-  const int hit_bytes = coop.empty() ? 0 : 8 * kHitCap + 16;  // candidates, hits, two counters
-  const int col_block = n_stages * stage_bytes + hit_bytes;
-  int dynamic_smem = col_block * (BT / 32) * n_varlen;
-  const int n_out = spec.kind == KernelKind::kProject ? static_cast<int>(exprs.size()) : 0;
-  const bool has_sel = spec.kind == KernelKind::kProject && spec.selection_mode != GDV_SEL_NONE;
-
-  // ---- TMA loader (projector, fixed-width inputs, no selection vector) -------------------------
-  // Each CTA tile (BT * R rows) of every input column is copied into a shared-memory stage by one
-  // cp.async.bulk; S stages per CTA keep (S - 1) tiles in flight per CTA while one computes.
-  // Picked by default for wide rows (>= 48 B of inputs), where the direct path runs out of
-  // registers before it has enough loads in flight.
-  bool staged = want_staged && (BT * R) % 128 == 0;
-  std::vector<int> val_off(slots.size(), 0), vld_off(slots.size(), 0);
-  int stage_total = 0, val_tx = 0, S = 0;
-  const int vld_copy = BT * R / 8 + 32;
-  if (staged) {
-    int o = 0;
-    for (size_t j = 0; j < slots.size(); ++j) {
-      val_off[j] = o;
-      o += BT * R * slots[j].type.width() + 16;
-      val_tx += BT * R * slots[j].type.width() + 16;
-    }
-    if (spec.nullable)
-      for (size_t j = 0; j < slots.size(); ++j) {
-        vld_off[j] = o;
-        o += vld_copy;
-      }
-    stage_total = (o + 127) / 128 * 128;
-    S = spec.stages > 0 ? spec.stages : 4;
-    while (S > 2 && S * stage_total > 220 * 1024) --S;
-    if (S < 2 || S * stage_total > 220 * 1024) {
-      staged = false;
-    } else {
-      dynamic_smem = S * stage_total;
-    }
-  }
-  ArgsLayout L(static_cast<int>(slots.size()), n_out, HasDictionary(slots), HasView(slots));
-
-  std::string src;
-  src += "// generated by gandiva_b200 kernel fuser; one fused kernel per ";
-  src += (spec.kind == KernelKind::kProject ? "Projector" : "Filter");
-  src += spec.nullable ? " (inputs may carry validity bitmaps)\n" : " (no input has nulls)\n";
-  for (size_t i = 0; i < exprs.size(); ++i)
-    src += "// expr_" + std::to_string(i) + ": " + CommentSafe(exprs[i]->ToString()) + "\n";
-  if (gated) src += "// gated loads: " + std::to_string(gate.stages()) + " stages\n";
-  src += "#include \"gdv_device_lib.cuh\"\n";
-  src += EmitArgsStruct(L);
-  src += gated ? sgen.globals() : gen.globals();
-  const std::string sR = std::to_string(R), sBT = std::to_string(BT);
-  const std::string s32R = std::to_string(32 * R);
-  // Fixed-width filters are bandwidth-bound and want every warp slot of the SM: ask for
-  // 2048 / BT resident CTAs, which caps the kernel at 32 registers per thread (what it needs).
-  std::string bounds = sBT;
-  bool light = spec.kind == KernelKind::kFilter && n_varlen == 0 && BT >= 256 && 2048 % BT == 0 &&
-               !gen.uses_ctx() && body.size() < 6000;
-  for (const auto& sl : slots)  // 128-bit math and string functions over dictionary views want registers
-    light = light && !sl.type.is_decimal() && !sl.type.is_dict() && !sl.type.is_view();
-  if (light && W > 1 && gated) {
-    // the stage chain keeps more values live than the ungated group: hold the 48 warps per SM that
-    // the ungated kernel reaches at W > 1 (40 registers)
-    bounds += ", " + std::to_string(1536 / BT);
-    light = false;
-  }
-  if (W > 1) light = false;  // W chunks keep 2 W more registers
-  if (light) bounds += ", " + std::to_string(2048 / BT);
-  src += "extern \"C\" __global__ void __launch_bounds__(" + bounds + ") " + spec.name +
-         "(const __grid_constant__ gdv_args A) {\n";
-  src += "  const u32 lane = threadIdx.x & 31u;\n";
-  src += "  const u32 wid = threadIdx.x >> 5;\n";
-  src += "  gdv_ctx ctx;\n  ctx.err = A.err;\n";
-  EmitPrologue(slots, spec, &src);
-  src += gated ? sgen.ScratchDecl(R) : gen.ScratchDecl(R);
-  if (stage_bytes > 0) {
-    src += "  extern __shared__ uint4 gdv_smem[];\n";
-    int vi = 0;
-    for (size_t j = 0; j < slots.size(); ++j) {
-      if (!HasByteRun(slots[j])) continue;
-      const std::string SJ = "stage" + std::to_string(j) + (prefetch ? "_0" : "");
-      src += "  u8* const " + SJ + " = reinterpret_cast<u8*>(gdv_smem) + ((size_t)wid * " +
-             std::to_string(n_varlen) + " + " + std::to_string(vi) + ") * " +
-             std::to_string(col_block) + ";\n";
-      if (SlotHasCoop(coop, static_cast<int>(j))) {
-        src += "  u32* cand" + std::to_string(j) + " = reinterpret_cast<u32*>(" + SJ +
-               " + " + std::to_string(n_stages * stage_bytes) + ");\n";
-        src += "  u32* hits" + std::to_string(j) + " = cand" + std::to_string(j) + " + " +
-               std::to_string(kHitCap) + ";\n";
-        src += "  u32* hctr" + std::to_string(j) + " = hits" + std::to_string(j) + " + " +
-               std::to_string(kHitCap) + ";  // [0] hits, [1] candidates\n";
-      }
-      ++vi;
-    }
-  }
-
-  if (spec.kind == KernelKind::kProject) {
-    for (int o = 0; o < n_out; ++o) {
-      const DataType& t = exprs[o]->result().type;
-      const std::string O = std::to_string(o);
-      if (!t.is_bool())
-        src += "  " + std::string(t.ctype()) + "* out" + O + " = reinterpret_cast<" + t.ctype() +
-               "*>(A.out_val[" + O + "]);\n";
-    }
-    // per-step tails: stores + validity / bool-data ballots
-    auto tail = [&](bool fast) {
-      std::string t5;
-      for (int o = 0; o < n_out; ++o) {
-        const DataType& t = exprs[o]->result().type;
-        const std::string O = std::to_string(o);
-        if (t.is_bool()) {
-          t5 += "        { const u32 m = __ballot_sync(GDV_FULL, in && (" + results[o].v +
-                ")); if (lane == (u32)k) dw" + O + " = m; }\n";
-        } else if (fast) {
-          t5 += "        gdv_stp(out" + O + " + s, (" + std::string(t.ctype()) + ")(" + results[o].v +
-                "));\n";
-        } else {
-          t5 += "        if (in) gdv_stp(out" + O + " + s, (" + std::string(t.ctype()) + ")(" +
-                results[o].v + "));\n";
-        }
-        t5 += "        { const u32 m = __ballot_sync(GDV_FULL, in && (" + results[o].ok +
-              ")); if (lane == (u32)k) vw" + O + " = m; }\n";
-      }
-      return t5;
-    };
-    const int NWP = BT / 32;
-    const int T = BT * R;  // rows per CTA tile
-    std::string wt_first = "0";
-    if (staged) {
-      // ---- TMA-staged full tiles: persistent CTAs, S stages, one bulk copy per column and tile
-      const std::string sS = std::to_string(S), sT = std::to_string(T);
-      src += "  extern __shared__ uint4 gdv_smem[];\n";
-      src += "  __shared__ u64 gdv_full[" + sS + "];\n";
-      src += "  u8* const stage0 = reinterpret_cast<u8*>(gdv_smem);\n";
-      std::string tx = std::to_string(val_tx) + "u";
-      for (size_t j = 0; j < slots.size(); ++j) {
-        const std::string J = std::to_string(j);
-        src += "  const u32 mis" + J + " = (u32)((unsigned long long)in_val" + J + " & 15ull);\n";
-        if (spec.nullable) {
-          src += "  const u32 vmis" + J + " = (u32)((unsigned long long)in_vld" + J + " & 15ull);\n";
-          tx += " + (in_hv" + J + " ? " + std::to_string(vld_copy) + "u : 0u)";
-        }
-      }
-      src += "  const u32 tx_bytes = " + tx + ";\n";
-      src += "  const u64 pol = gdv_policy_evict_first();\n";
-      // a bulk copy may read up to 32 bytes past its tile: the last 256 rows are never staged
-      src += "  const i64 n_st = A.n > 256 ? (A.n - 256) / " + sT + " : 0;\n";
-      src += "  if (threadIdx.x == 0) {\n";
-      src += "    for (u32 s = 0; s < " + sS + "u; ++s) gdv_mbar_init(&gdv_full[s], 1u);\n";
-      src += "    gdv_fence_mbar_init();\n";
-      src += "  }\n";
-      src += "  __syncthreads();\n";
-      src += "  auto issue = [&](i64 t, u32 s) {\n";
-      src += "    u8* sb = stage0 + (size_t)s * " + std::to_string(stage_total) + "u;\n";
-      src += "    gdv_mbar_expect_tx(&gdv_full[s], tx_bytes);\n";
-      for (size_t j = 0; j < slots.size(); ++j) {
-        const std::string J = std::to_string(j);
-        const int w = slots[j].type.width();
-        src += "    gdv_bulk_g2s(sb + " + std::to_string(val_off[j]) + ", reinterpret_cast<const u8*>(in_val" +
-               J + ") - mis" + J + " + t * " + std::to_string(static_cast<long long>(T) * w) + "ll, " +
-               std::to_string(T * w + 16) + "u, &gdv_full[s], pol);\n";
-        if (spec.nullable)
-          src += "    if (in_hv" + J + ") gdv_bulk_g2s(sb + " + std::to_string(vld_off[j]) +
-                 ", reinterpret_cast<const u8*>(in_vld" + J + ") - vmis" + J + " + t * " +
-                 std::to_string(T / 8) + "ll, " + std::to_string(vld_copy) + "u, &gdv_full[s], pol);\n";
-      }
-      src += "  };\n";
-      src += "  if (threadIdx.x == 0) {\n";
-      src += "    for (u32 s = 0; s < " + sS + "u; ++s) {\n";
-      src += "      const i64 t = (i64)blockIdx.x + (i64)s * gridDim.x;\n";
-      src += "      if (t < n_st) issue(t, s);\n";
-      src += "    }\n";
-      src += "  }\n";
-      src += "  u32 it = 0u;\n";
-      src += "  for (i64 t = blockIdx.x; t < n_st; t += gridDim.x, ++it) {\n";
-      src += "    const u32 s = it % " + sS + "u;\n";
-      src += "    const u32 par = (it / " + sS + "u) & 1u;\n";
-      src += "    const u8* sb = stage0 + (size_t)s * " + std::to_string(stage_total) + "u;\n";
-      src += "    const i64 base = t * " + sT + " + (i64)wid * " + s32R + ";\n";
-      for (size_t j = 0; j < slots.size(); ++j) {
-        const std::string J = std::to_string(j);
-        const std::string ct = slots[j].type.ctype();
-        src += "    const " + ct + "* sp" + J + " = reinterpret_cast<const " + ct + "*>(sb + " +
-               std::to_string(val_off[j]) + " + mis" + J + ") + wid * " + s32R + "u + lane;\n";
-        if (spec.nullable)
-          src += "    const u32* sv" + J + " = reinterpret_cast<const u32*>(sb + " +
-                 std::to_string(vld_off[j]) + " + vmis" + J + ");\n";
-      }
-      for (int o = 0; o < n_out; ++o) {
-        src += "    u32 vw" + std::to_string(o) + " = 0u;\n";
-        if (exprs[o]->result().type.is_bool()) src += "    u32 dw" + std::to_string(o) + " = 0u;\n";
-      }
-      src += "    gdv_mbar_wait(&gdv_full[s], par);\n";
-      src += "    {\n";
-      std::string after;
-      after += "      __syncthreads();  // every thread holds its rows: the stage can be refilled\n";
-      after += "      if (threadIdx.x == 0) {\n";
-      after += "        const i64 tn = t + (i64)" + sS + " * gridDim.x;\n";
-      after += "        if (tn < n_st) issue(tn, s);\n";
-      after += "      }\n";
-      EmitGroup(slots, spec, R, kStaged, body, tail(true), &src, 3, 0, after, coop);
-      src += "    }\n";
-      src += "    if (lane < " + sR + "u) {\n";
-      src += "      const i64 w = (base >> 5) + (i64)lane;\n";
-      for (int o = 0; o < n_out; ++o) {
-        const std::string O = std::to_string(o);
-        src += "      if (A.out_vld[" + O + "] != nullptr) A.out_vld[" + O + "][w] = vw" + O + ";\n";
-        if (exprs[o]->result().type.is_bool())
-          src += "      reinterpret_cast<u32*>(A.out_val[" + O + "])[w] = dw" + O + ";\n";
-      }
-      src += "    }\n";
-      src += "  }\n";
-      // rows after the staged tiles take the direct path below
-      wt_first = "n_st * " + std::to_string(NWP);
-    }
-    src += "  const i64 n_wtiles = (A.n + " + std::to_string(32 * R - 1) + ") / " + s32R + ";\n";
-    src += "  const i64 wstride = (i64)gridDim.x * " + std::to_string(NWP) + ";\n";
-    src += "  for (i64 wt = " + wt_first + " + (i64)blockIdx.x * " + std::to_string(NWP) +
-           " + wid; wt < n_wtiles; wt += wstride) {\n";
-    src += "    const i64 base = wt * " + s32R + ";\n";
-    for (int o = 0; o < n_out; ++o) {
-      src += "    u32 vw" + std::to_string(o) + " = 0u;\n";
-      if (exprs[o]->result().type.is_bool()) src += "    u32 dw" + std::to_string(o) + " = 0u;\n";
-    }
-    if (!has_sel) {
-      src += "    if (base + " + s32R + " <= A.n) {\n";
-      EmitGroup(slots, spec, R, kFast, body, tail(true), &src, 3, stage_bytes, std::string(), coop);
-      src += "    } else {\n";
-      EmitGroup(slots, spec, R, kPred, body, tail(false), &src, 3, 0, std::string(), coop);
-      src += "    }\n";
-    } else {
-      src += "    {\n";
-      EmitGroup(slots, spec, R, kPred, body, tail(false), &src, 3, 0, std::string(), coop);
-      src += "    }\n";
-    }
-    src += "    if (lane < " + sR + "u && base + 32 * (i64)lane < A.n) {\n";
-    src += "      const i64 w = (base >> 5) + (i64)lane;\n";
-    for (int o = 0; o < n_out; ++o) {
-      const std::string O = std::to_string(o);
-      src += "      if (A.out_vld[" + O + "] != nullptr) A.out_vld[" + O + "][w] = vw" + O + ";\n";
-      if (exprs[o]->result().type.is_bool())
-        src += "      reinterpret_cast<u32*>(A.out_val[" + O + "])[w] = dw" + O + ";\n";
-    }
-    src += "    }\n";
-    src += "  }\n";
-    src += "}\n";
-  } else {
-    // Filter: every warp owns 1024 consecutive rows per chunk (32 steps of 32 rows).  Step k's
-    // keep-mask is one ballot word, parked in lane k, so a chunk costs one register per thread
-    // regardless of its size; loads are issued R steps at a time for memory-level parallelism.
-    // Large tiles keep the number of look-back descriptors per launch small, which is what bounds
-    // ordered compaction at HBM bandwidth (DESIGN.md "Filter kernel").
-    const std::string IDX = SelCType(spec.selection_mode);
-    const int NW = BT / 32;
-    const int WT = NW * 1024 * W;
-    const std::string sW = std::to_string(W);
-    src += "  __shared__ u32 s_wcount[" + std::to_string(NW) + "];\n";
-    src += "  __shared__ i64 s_tile;\n";
-    src += "  __shared__ u64 s_excl;\n";
-    src += "  const i64 n_tiles = (A.n + " + std::to_string(WT - 1) + ") / " + std::to_string(WT) + ";\n";
-    src += "  " + IDX + "* out_idx = reinterpret_cast<" + IDX + "*>(A.out_idx);\n";
-    src += "  const u32 lt = gdv_lanemask_lt();\n";
-    src += "  while (true) {\n";
-    src += "    if (threadIdx.x == 0) s_tile = (i64)atomicAdd(A.ticket, 1ull);\n";
-    src += "    __syncthreads();\n";
-    src += "    const i64 tile = s_tile;\n";
-    src += "    if (tile >= n_tiles) break;\n";
-    src += "    const i64 wbase0 = tile * " + std::to_string(WT) + " + (i64)wid * " + std::to_string(1024 * W) + ";\n";
-    src += "    u32 mymask[" + sW + "];\n";
-    const std::string step_tail =
-        "          { const u32 m = __ballot_sync(GDV_FULL, in && (" + results[0].ok + ") && (" +
-        results[0].v + ")); if (lane == (u32)(g + k)) cur = m; }\n";
-    if (n_varlen == 0) {
-      // Fixed-width columns.  Every warp walks W consecutive 1024-row chunks per tile, so a
-      // 32K-row tile needs 256 threads at W = 4 and eight small CTAs share an SM: while one sits in
-      // its tile-end barriers and look-back, seven keep streaming.
-      src += "    #pragma unroll\n";
-      src += "    for (int w = 0; w < " + sW + "; ++w) {\n";
-      src += "      const i64 wbase = wbase0 + 1024 * w;\n";
-      src += "      u32 cur = 0u;\n";
-      src += "      #pragma unroll 1\n";
-      src += "      for (int g = 0; g < 32; g += " + sR + ") {\n";
-      src += "        const i64 base = wbase + 32 * g;\n";
-      src += "        if (base >= A.n) break;\n";
-      src += "        if (base + " + s32R + " <= A.n) {\n";
-      const std::string gated_tail =
-          "          { const u32 m = __ballot_sync(GDV_FULL, in && alive[k]); if (lane == (u32)(g + k)) cur = m; }\n";
-      if (gated)
-        EmitGatedGroup(slots, spec, R, kFast, gate, gate_seg, gated_tail, &src, 5);
-      else
-        EmitGroup(slots, spec, R, kFast, body, step_tail, &src, 5, 0, std::string(), coop);
-      src += "        } else {\n";
-      if (gated)
-        EmitGatedGroup(slots, spec, R, kPred, gate, gate_seg, gated_tail, &src, 5);
-      else
-        EmitGroup(slots, spec, R, kPred, body, step_tail, &src, 5, 0, std::string(), coop);
-      src += "        }\n";
-      src += "      }\n";
-      src += "      mymask[w] = cur;\n";
-      src += "    }\n";
-    } else {
-      // String columns: one 1024-row chunk per warp; the bytes of the NEXT group are copied into a
-      // second shared-memory stage with cp.async while the current group is scanned.
-      src += "    const i64 wbase = wbase0;\n";
-      src += "    u32 cur = 0u;\n";
-      // issue(b, par): cp.async the bytes of the full group that starts at row b into stage `par`
-      src += "    auto issue = [&](i64 b, u32 par) {\n";
-      for (size_t j = 0; j < slots.size(); ++j) {
-        if (!HasByteRun(slots[j])) continue;
-        const std::string J = std::to_string(j);
-        src += "      {\n";
-        src += "        const i32 gb = in_val" + J + "[b];\n";
-        src += "        const i32 gn = in_val" + J + "[b + " + s32R + "] - gb;\n";
-        src += "        const u8* src = in_var" + J + " + gb;\n";
-        src += "        const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
-        src += "        if (gn + (i32)mis <= " + std::to_string(stage_bytes) + ") {\n";
-        src += "          const i32 nchunks = (gn + (i32)mis + 15) >> 4;\n";
-        src += "          u8* dst = stage" + J + "_0 + (size_t)par * " + std::to_string(stage_bytes) + "u;\n";
-        src += "          for (i32 c = (i32)lane; c < nchunks; c += 32)\n";
-        src += "            gdv_cp_async16(dst + 16 * c, src - mis + 16 * c);\n";
-        src += "        }\n";
-        src += "      }\n";
-      }
-      src += "      gdv_cp_async_commit();\n";
-      src += "    };\n";
-      src += "    u32 par = 0u;\n";
-      src += "    if (wbase + " + s32R + " <= A.n) issue(wbase, 0u);\n";
-      src += "    #pragma unroll 1\n";
-      src += "    for (int g = 0; g < 32; g += " + sR + ") {\n";
-      src += "      const i64 base = wbase + 32 * g;\n";
-      src += "      if (base >= A.n) break;\n";
-      for (size_t j = 0; j < slots.size(); ++j)
-        if (HasByteRun(slots[j]))
-          src += "      u8* const stage" + std::to_string(j) + " = stage" + std::to_string(j) +
-                 "_0 + (size_t)par * " + std::to_string(stage_bytes) + "u;\n";
-      src += "      if (base + " + s32R + " <= A.n) {\n";
-      src += "        if (g + " + sR + " < 32 && base + " + std::to_string(64 * R) + " <= A.n) {\n";
-      src += "          issue(base + " + s32R + ", par ^ 1u);\n";
-      src += "          gdv_cp_async_wait<1>();\n";
-      src += "        } else {\n";
-      src += "          gdv_cp_async_wait<0>();\n";
-      src += "        }\n";
-      src += "        __syncwarp();\n";
-      src += "        par ^= 1u;\n";
-      EmitGroup(slots, spec, R, kFast, body, step_tail, &src, 4, stage_bytes, std::string(), coop, true);
-      src += "      } else {\n";
-      EmitGroup(slots, spec, R, kPred, body, step_tail, &src, 4, 0, std::string(), coop);
-      src += "      }\n";
-      src += "    }\n";
-      src += "    mymask[0] = cur;\n";
-    }
-    EmitFilterEpilogue(slots, spec, NW, W, IDX, &src);
-    src += "  }\n";
-    src += "}\n";
-  }
-
-  if (has_sel) ApplyDeviceCount(&src);
-  out->source = std::move(src);
-  out->name = spec.name;
-  out->kind = spec.kind;
-  out->rows_per_thread = R;
-  out->block_threads = BT;
-  out->selection_mode = spec.selection_mode;
-  out->nullable = spec.nullable;
-  out->inputs = slots;
-  out->outputs.clear();
-  if (spec.kind == KernelKind::kProject)
-    for (const auto& e : exprs) out->outputs.push_back(e->result().type);
-  out->uses_ctx = gen.uses_ctx();
-  out->in_bytes_per_row = in_bytes;
-  out->out_bytes_per_row = out_bytes;
-  out->args_size = L.size;
-  out->dynamic_smem = dynamic_smem;
-  out->tile_rows = spec.kind == KernelKind::kFilter ? static_cast<int64_t>(BT / 32) * 1024 * W : 0;
-  out->staged = staged;
-  out->stages = staged ? S : 0;
-  out->cta_tile_rows = static_cast<int64_t>(BT) * R;
-  out->view_shortcuts = gen.view_shortcuts();
-  out->gated_stages = gated ? gate.stages() : 0;
-  return Status::OK();
+  if (s.kind == KernelKind::kProject) return GenerateProjector(schema, lowered, s, out);
+  if (GenerateKeyFilter(schema, lowered, s, out)) return Status::OK();
+  return GenerateFilter(schema, lowered, s, out);
 }
-
-}  // namespace
 
 }  // namespace gdv

@@ -59,30 +59,6 @@ struct ColumnSlot {
   bool hoist = false;
 };
 
-struct GeneratedKernel {
-  std::string source;   // full translation unit (device library is #include'd by name)
-  std::string name;
-  KernelKind kind;
-  int rows_per_thread;
-  int block_threads;
-  int selection_mode;
-  bool nullable = true;
-  std::vector<ColumnSlot> inputs;   // kernel input slot j reads schema column inputs[j]
-  std::vector<DataType> outputs;    // project: one per expression; filter: empty
-  bool uses_ctx = false;            // some function can raise an ExecutionError
-  int in_bytes_per_row = 0;         // algorithmic bytes (values only) read per row
-  int out_bytes_per_row = 0;
-  size_t args_size = 0;             // sizeof(gdv_args) for this kernel
-  int dynamic_smem = 0;             // bytes of dynamic shared memory (string staging)
-  int64_t tile_rows = 0;            // filter: rows per CTA tile (one look-back descriptor each)
-  bool key_driven = false;          // string filter driven by the occurrences of a literal key in the column's bytes
-  bool staged = false;              // project: inputs staged through shared memory by TMA bulk copies
-  int stages = 0;                   // staged: shared-memory stages per CTA
-  int64_t cta_tile_rows = 0;        // staged: rows per CTA tile (block_threads * rows_per_thread)
-  int view_shortcuts = 0;           // call sites decided from the raw 16-byte views (BodyGen::ViewShortcut)
-  int gated_stages = 0;             // fixed-width filter: stages of gated loads (GatePlan), 0 = not gated
-};
-
 // Byte offsets inside gdv_args; the host packs the same layout (see EmitArgsStruct()).
 struct ArgsLayout {
   int ni, no;  // array extents (>= 1)
@@ -100,6 +76,32 @@ struct ArgsLayout {
   bool view = false;
   size_t off_in_vbf = 0, off_in_vsz = 0, off_in_vbn = 0;
   ArgsLayout(int n_inputs, int n_outputs, bool dictionary = false, bool views = false);
+};
+
+// What the fuser generated, and how the runtime launches it.  Fields a kernel shape does not use
+// keep their defaults.
+struct GeneratedKernel {
+  std::string source;   // full translation unit (device library is #include'd by name)
+  std::string name;
+  KernelKind kind = KernelKind::kProject;
+  int rows_per_thread = 0;
+  int block_threads = 0;
+  int selection_mode = GDV_SEL_NONE;
+  bool nullable = true;
+  std::vector<ColumnSlot> inputs;   // kernel input slot j reads schema column inputs[j]
+  std::vector<DataType> outputs;    // project: one per expression; filter: empty
+  bool uses_ctx = false;            // some function can raise an ExecutionError
+  int in_bytes_per_row = 0;         // algorithmic bytes (values only) read per row
+  int out_bytes_per_row = 0;
+  ArgsLayout args{0, 0};            // the gdv_args layout the kernel was emitted with; the host packs it
+  int dynamic_smem = 0;             // bytes of dynamic shared memory (string staging)
+  int64_t tile_rows = 0;            // filter: rows per CTA tile (one look-back descriptor each)
+  bool key_driven = false;          // string filter driven by the occurrences of a literal key in the column's bytes
+  bool staged = false;              // project: inputs staged through shared memory by TMA bulk copies
+  int stages = 0;                   // staged: shared-memory stages per CTA
+  int64_t cta_tile_rows = 0;        // staged: rows per CTA tile (block_threads * rows_per_thread)
+  int view_shortcuts = 0;           // call sites decided from the raw 16-byte views (BodyGen::ViewShortcut)
+  int gated_stages = 0;             // fixed-width filter: stages of gated loads (GatePlan), 0 = not gated
 };
 
 bool HasDictionary(const std::vector<ColumnSlot>& slots);

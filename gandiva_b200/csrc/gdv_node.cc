@@ -229,4 +229,36 @@ std::string InNode::ToString() const {
   return ss.str();
 }
 
+NodeVector Children(const Node& node) {
+  switch (node.kind()) {
+    case NodeKind::kFunction: return static_cast<const FunctionNode&>(node).children();
+    case NodeKind::kIf: {
+      const auto& n = static_cast<const IfNode&>(node);
+      return {n.condition(), n.then_node(), n.else_node()};
+    }
+    case NodeKind::kBoolean: return static_cast<const BooleanNode&>(node).children();
+    case NodeKind::kIn: return {static_cast<const InNode&>(node).child()};
+    default: return {};
+  }
+}
+
+NodePtr WithChildren(const NodePtr& node, NodeVector children) {
+  if (children == Children(*node)) return node;
+  switch (node->kind()) {
+    case NodeKind::kFunction: {
+      const auto& fn = static_cast<const FunctionNode&>(*node);
+      return std::make_shared<FunctionNode>(fn.name(), std::move(children), fn.return_type());
+    }
+    case NodeKind::kIf:
+      return std::make_shared<IfNode>(children[0], children[1], children[2], node->return_type());
+    case NodeKind::kBoolean:
+      return std::make_shared<BooleanNode>(static_cast<const BooleanNode&>(*node).op(), std::move(children));
+    case NodeKind::kIn: {
+      const auto& n = static_cast<const InNode&>(*node);
+      return std::make_shared<InNode>(children[0], n.value_type(), n.ints(), n.strs());
+    }
+    default: return node;
+  }
+}
+
 }  // namespace gdv

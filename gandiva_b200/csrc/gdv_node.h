@@ -126,6 +126,13 @@ class InNode : public Node {
   std::vector<std::string> strs_;
 };
 
+// The children of a node in evaluation order (an If's condition, then, else); none for fields and
+// literals.  Walks that treat every kind of node alike go through these two instead of a switch.
+NodeVector Children(const Node& node);
+// The same node over `children` (as many as Children(*node) returns).  Returns `node` itself when no
+// child pointer changed.
+NodePtr WithChildren(const NodePtr& node, NodeVector children);
+
 struct Field {
   std::string name;
   DataType type;

@@ -114,36 +114,18 @@ struct Extractor {
           return std::make_shared<FunctionNode>(fn.name(), std::move(kids), fn.return_type());
         }
         NodeVector kids;
-        bool changed = false;
-        for (const auto& c : fn.children()) {
-          kids.push_back(Walk(c, is_concat));
-          changed = changed || kids.back() != c;
-        }
-        return changed ? std::make_shared<FunctionNode>(fn.name(), std::move(kids), fn.return_type()) : node;
+        for (const auto& c : fn.children()) kids.push_back(Walk(c, is_concat));
+        return WithChildren(node, std::move(kids));
       }
       case NodeKind::kIf: {
         const auto& n = static_cast<const IfNode&>(*node);
-        const NodePtr c = Walk(n.condition(), false), t = Walk(n.then_node(), rope_ok), e = Walk(n.else_node(), rope_ok);
-        if (c == n.condition() && t == n.then_node() && e == n.else_node()) return node;
-        return std::make_shared<IfNode>(c, t, e, n.return_type());
+        return WithChildren(node, {Walk(n.condition(), false), Walk(n.then_node(), rope_ok), Walk(n.else_node(), rope_ok)});
       }
-      case NodeKind::kBoolean: {
-        const auto& n = static_cast<const BooleanNode&>(*node);
+      default: {  // and / or / IN read no rope
         NodeVector kids;
-        bool changed = false;
-        for (const auto& c : n.children()) {
-          kids.push_back(Walk(c, false));
-          changed = changed || kids.back() != c;
-        }
-        return changed ? std::make_shared<BooleanNode>(n.op(), std::move(kids)) : node;
+        for (const auto& c : Children(*node)) kids.push_back(Walk(c, false));
+        return WithChildren(node, std::move(kids));
       }
-      case NodeKind::kIn: {
-        const auto& n = static_cast<const InNode&>(*node);
-        const NodePtr c = Walk(n.child(), false);
-        return c == n.child() ? node : std::make_shared<InNode>(c, n.value_type(), n.ints(), n.strs());
-      }
-      default:
-        return node;
     }
   }
 };

@@ -422,11 +422,34 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
     g_cubin_cache.emplace(key, std::move(entry));
   }
   // GDV_DUMP_DIR=<dir>: write <kernel>.cu / <kernel>.cubin for offline SASS inspection
-  // (cuobjdump -sass) and so that ncu's source page can find the generated code.
+  // (cuobjdump -sass) and so that ncu's source page can find the generated code, and <kernel>.info
+  // with the launch fields the fuser chose (one key=value per line), so that two versions of the
+  // fuser can be compared kernel by kernel.
   if (const char* dir = std::getenv("GDV_DUMP_DIR")) {
     const std::string base = std::string(dir) + "/" + k->gen.name;
     if (FILE* f = std::fopen((base + ".cu").c_str(), "w")) {
       std::fwrite(k->gen.source.data(), 1, k->gen.source.size(), f);
+      std::fclose(f);
+    }
+    if (FILE* f = std::fopen((base + ".info").c_str(), "w")) {
+      const GeneratedKernel& g = k->gen;
+      std::fprintf(f, "rows_per_thread=%d\nblock_threads=%d\nselection_mode=%d\nnullable=%d\n", g.rows_per_thread,
+                   g.block_threads, g.selection_mode, g.nullable ? 1 : 0);
+      for (size_t j = 0; j < g.inputs.size(); ++j) {
+        const gdv_type_t t = g.inputs[j].type.c();
+        std::fprintf(f, "input%zu=col %d type %d/%d/%d hoist %d\n", j, g.inputs[j].schema_index, t.id, t.precision,
+                     t.scale, g.inputs[j].hoist ? 1 : 0);
+      }
+      for (size_t o = 0; o < g.outputs.size(); ++o) {
+        const gdv_type_t t = g.outputs[o].c();
+        std::fprintf(f, "output%zu=type %d/%d/%d\n", o, t.id, t.precision, t.scale);
+      }
+      std::fprintf(f, "uses_ctx=%d\nin_bytes_per_row=%d\nout_bytes_per_row=%d\nargs_size=%zu\ndynamic_smem=%d\n",
+                   g.uses_ctx ? 1 : 0, g.in_bytes_per_row, g.out_bytes_per_row, g.args.size, g.dynamic_smem);
+      std::fprintf(f, "tile_rows=%lld\nkey_driven=%d\nstaged=%d\nstages=%d\ncta_tile_rows=%lld\n",
+                   static_cast<long long>(g.tile_rows), g.key_driven ? 1 : 0, g.staged ? 1 : 0, g.stages,
+                   static_cast<long long>(g.cta_tile_rows));
+      std::fprintf(f, "view_shortcuts=%d\ngated_stages=%d\n", g.view_shortcuts, g.gated_stages);
       std::fclose(f);
     }
     if (FILE* f = std::fopen((base + ".cubin").c_str(), "wb")) {
@@ -1049,7 +1072,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   scratch.Guard(stream);
   std::vector<ResolvedIn> ins;
   GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), 1, HasDictionary(gen.inputs), HasView(gen.inputs));
+  const ArgsLayout& L = gen.args;
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
   PutInputs(args, L, ins);
@@ -1216,7 +1239,7 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
   GDV_RETURN_NOT_OK(ResolveInputs(dev, gen, batch, stream, &scratch, &ins));
   const double t_inputs = TraceOn() ? NowUs() : 0.0;
 
-  ArgsLayout L(static_cast<int>(gen.inputs.size()), n_outs, HasDictionary(gen.inputs), HasView(gen.inputs));
+  const ArgsLayout& L = gen.args;
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
   PutInputs(args, L, ins);
@@ -1481,7 +1504,8 @@ Status Filter::KernelFor(int mode, bool nullable, bool large, CompiledKernel** o
     std::unique_ptr<CompiledKernel> k;
     std::vector<ExpressionPtr> exprs = {cond_};
     // Big batches want big tiles (few look-back descriptors), small ones enough tiles to occupy the
-    // 132 SMs: the fuser picks block size and chunks per warp from this flag (GenerateKernelImpl).
+    // 132 SMs: the fuser picks block size and chunks per warp from this flag (GenerateKeyFilter,
+    // GenerateFilter and FitStages in gdv_codegen.cc).
     Config cfg = cfg_;
     cfg.large_batch = large;
     GDV_RETURN_NOT_OK(BuildKernel(*schema_, exprs, KernelKind::kFilter, mode, nullable, cfg, &k));
@@ -1617,7 +1641,7 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
                                             out_sel->index_base, bounded ? out_sel->max_slots : n, &scratch));
   } else {
     const GeneratedKernel& gen = kernel->gen;
-    ArgsLayout L(static_cast<int>(gen.inputs.size()), 0, HasDictionary(gen.inputs), HasView(gen.inputs));
+    const ArgsLayout& L = gen.args;
     std::vector<uint8_t> args(L.size, 0);
     Put<int64_t>(args, L.off_n, n);
     Put<int64_t>(args, L.off_row_base, out_sel->index_base);
