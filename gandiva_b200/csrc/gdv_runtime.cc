@@ -106,8 +106,6 @@ Status Device::Get(int ordinal, Device** out) {
     d.DeviceGetAttribute(&dev->cc_minor_, CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MINOR, dev->dev_);
     GDV_RETURN_NOT_OK(
         CuCheck(d.StreamCreate(&dev->stream_, CU_STREAM_NON_BLOCKING), "cuStreamCreate"));
-    GDV_RETURN_NOT_OK(
-        CuCheck(d.StreamCreate(&dev->copy_stream_, CU_STREAM_NON_BLOCKING), "cuStreamCreate"));
     dev->owner_thread_ = std::this_thread::get_id();
     if (const char* lim = std::getenv("GDV_POOL_LIMIT_MB")) dev->pool_limit_ = static_cast<size_t>(std::atoll(lim)) << 20;
     g_devices[ordinal] = dev.release();
@@ -169,17 +167,7 @@ Status Device::Alloc(size_t bytes, CUdeviceptr* out) {
   CUresult r = Driver().MemAlloc(&p, want);
   if (r == CUDA_ERROR_OUT_OF_MEMORY) {
     // drop the cache and retry once
-    std::vector<CUdeviceptr> drop;
-    {
-      std::lock_guard<std::mutex> lock(mu_);
-      for (auto& kv : free_) {
-        drop.push_back(kv.second);
-        sizes_.erase(kv.second);
-      }
-      free_.clear();
-      idle_bytes_ = 0;
-    }
-    for (auto q : drop) Driver().MemFree(q);
+    Trim(0);
     r = Driver().MemAlloc(&p, want);
   }
   if (r != CUDA_SUCCESS) {
@@ -197,25 +185,17 @@ Status Device::Alloc(size_t bytes, CUdeviceptr* out) {
 
 void Device::Free(CUdeviceptr p) {
   if (p == 0) return;
-  std::vector<CUdeviceptr> drop;
   {
     std::lock_guard<std::mutex> lock(mu_);
     auto it = sizes_.find(p);
     if (it == sizes_.end()) return;
     free_.emplace(it->second, p);
     idle_bytes_ += it->second;
-    // over the limit: the largest idle blocks go back to the driver (cuMemFree waits for work that
-    // still uses a block, so releasing one that a queued kernel reads is safe, only slow)
-    while (idle_bytes_ > pool_limit_ && !free_.empty()) {
-      auto big = std::prev(free_.end());
-      idle_bytes_ -= big->first;
-      sizes_.erase(big->second);
-      drop.push_back(big->second);
-      free_.erase(big);
-    }
+    if (idle_bytes_ <= pool_limit_) return;
   }
-  if (!drop.empty() && MakeCurrent().ok())
-    for (auto q : drop) Driver().MemFree(q);
+  // over the limit: the largest idle blocks go back to the driver (cuMemFree waits for work that
+  // still uses a block, so releasing one that a queued kernel reads is safe, only slow)
+  Trim(pool_limit_);
 }
 
 size_t Device::Trim(size_t keep_bytes) {
@@ -320,6 +300,103 @@ const char* KernelPrefix(KernelKind kind) {
   }
 }
 
+std::string Hex64(uint64_t h) {
+  char hex[24];
+  std::snprintf(hex, sizeof(hex), "%016llx", static_cast<unsigned long long>(h));
+  return hex;
+}
+
+// The device function library is part of every translation unit: its text is part of the key, so a
+// persisted cubin can never outlive the library it was compiled against.
+std::string CubinKey(const std::string& arch, const Config& cfg, const std::string& source) {
+  static const std::string lib_hex =
+      Hex64(Fnv1a(std::string(gdv_device_lib_text, static_cast<size_t>(gdv_device_lib_text_len))));
+  return arch + (cfg.optimize ? "|O3|" : "|O0|") + (cfg.dump_ir ? "ptx|" : "|") + lib_hex + "|" + source;
+}
+
+void RememberCubin(const std::string& key, std::shared_ptr<const CachedCubin> entry) {
+  std::lock_guard<std::mutex> lock(g_cache_mu);
+  if (g_cubin_cache.size() >= kCubinCacheEntries) g_cubin_cache.clear();
+  g_cubin_cache.emplace(key, std::move(entry));
+}
+
+// GDV_CUBIN_CACHE_DIR=<dir>: cubins also persist across processes (the counterpart of the
+// reference's object-code cache): <dir>/<fnv64 of arch|options|source>.cubin, written atomically.
+// Empty when off, and with dump_ir: DumpIR wants the PTX too, so that always compiles.
+std::string DiskCachePath(const std::string& key, const Config& cfg) {
+  const char* cdir = std::getenv("GDV_CUBIN_CACHE_DIR");
+  if (cdir == nullptr || cfg.dump_ir) return "";
+  return std::string(cdir) + "/" + Hex64(Fnv1a(key)) + ".cubin";
+}
+
+bool IsElf(const std::vector<char>& b) {
+  return b.size() > 4 && b[0] == 0x7f && b[1] == 'E' && b[2] == 'L' && b[3] == 'F';
+}
+
+// The persisted cubin at `path` when it is an ELF image that holds kernel `name`, else null.
+std::shared_ptr<const CachedCubin> ReadDiskCubin(const std::string& path, const std::string& name) {
+  FILE* f = std::fopen(path.c_str(), "rb");
+  if (f == nullptr) return nullptr;
+  std::vector<char> blob;
+  char buf[65536];
+  size_t got;
+  while ((got = std::fread(buf, 1, sizeof(buf), f)) > 0) blob.insert(blob.end(), buf, buf + got);
+  std::fclose(f);
+  if (!IsElf(blob) || std::search(blob.begin(), blob.end(), name.begin(), name.end()) == blob.end()) return nullptr;
+  auto entry = std::make_shared<CachedCubin>();
+  entry->cubin = std::move(blob);
+  return entry;
+}
+
+// Written to a per-process temporary and renamed, so that a reader never sees half a file.
+void WriteDiskCubin(const std::string& path, const std::vector<char>& cubin) {
+  if (!IsElf(cubin)) return;
+  const std::string tmp = path + ".tmp" + std::to_string(static_cast<long long>(::getpid()));
+  FILE* f = std::fopen(tmp.c_str(), "wb");
+  if (f == nullptr) return;
+  const bool ok = std::fwrite(cubin.data(), 1, cubin.size(), f) == cubin.size();
+  std::fclose(f);
+  if (ok) std::rename(tmp.c_str(), path.c_str());
+  else std::remove(tmp.c_str());
+}
+
+// GDV_DUMP_DIR=<dir>: write <kernel>.cu / <kernel>.cubin for offline SASS inspection
+// (cuobjdump -sass) and so that ncu's source page can find the generated code, and <kernel>.info
+// with the launch fields the fuser chose (one key=value per line), so that two versions of the
+// fuser can be compared kernel by kernel.
+void DumpKernel(const char* dir, const CompiledKernel& k) {
+  const std::string base = std::string(dir) + "/" + k.gen.name;
+  if (FILE* f = std::fopen((base + ".cu").c_str(), "w")) {
+    std::fwrite(k.gen.source.data(), 1, k.gen.source.size(), f);
+    std::fclose(f);
+  }
+  if (FILE* f = std::fopen((base + ".info").c_str(), "w")) {
+    const GeneratedKernel& g = k.gen;
+    std::fprintf(f, "rows_per_thread=%d\nblock_threads=%d\nselection_mode=%d\nnullable=%d\n", g.rows_per_thread,
+                 g.block_threads, g.selection_mode, g.nullable ? 1 : 0);
+    for (size_t j = 0; j < g.inputs.size(); ++j) {
+      const gdv_type_t t = g.inputs[j].type.c();
+      std::fprintf(f, "input%zu=col %d type %d/%d/%d hoist %d\n", j, g.inputs[j].schema_index, t.id, t.precision,
+                   t.scale, g.inputs[j].hoist ? 1 : 0);
+    }
+    for (size_t o = 0; o < g.outputs.size(); ++o) {
+      const gdv_type_t t = g.outputs[o].c();
+      std::fprintf(f, "output%zu=type %d/%d/%d\n", o, t.id, t.precision, t.scale);
+    }
+    std::fprintf(f, "uses_ctx=%d\nin_bytes_per_row=%d\nout_bytes_per_row=%d\nargs_size=%zu\ndynamic_smem=%d\n",
+                 g.uses_ctx ? 1 : 0, g.in_bytes_per_row, g.out_bytes_per_row, g.args.size, g.dynamic_smem);
+    std::fprintf(f, "tile_rows=%lld\nkey_driven=%d\nstaged=%d\nstages=%d\ncta_tile_rows=%lld\n",
+                 static_cast<long long>(g.tile_rows), g.key_driven ? 1 : 0, g.staged ? 1 : 0, g.stages,
+                 static_cast<long long>(g.cta_tile_rows));
+    std::fprintf(f, "view_shortcuts=%d\ngated_stages=%d\n", g.view_shortcuts, g.gated_stages);
+    std::fclose(f);
+  }
+  if (FILE* f = std::fopen((base + ".cubin").c_str(), "wb")) {
+    std::fwrite(k.cubin.data(), 1, k.cubin.size(), f);
+    std::fclose(f);
+  }
+}
+
 Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs,
                    KernelKind kind, int selection_mode, bool nullable, const Config& cfg,
                    std::unique_ptr<CompiledKernel>* out) {
@@ -344,51 +421,21 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
   Device* dev = nullptr;
   if (Driver().loaded && Device::Get(cfg.device, &dev).ok()) arch = dev->arch();
   // name the kernel after its own text
-  char hex[24];
-  std::snprintf(hex, sizeof(hex), "%016llx", static_cast<unsigned long long>(Fnv1a(arch, Fnv1a(k->gen.source))));
-  const std::string name = std::string(KernelPrefix(kind)) + hex;
+  const std::string name = std::string(KernelPrefix(kind)) + Hex64(Fnv1a(arch, Fnv1a(k->gen.source)));
   for (size_t pos = 0; (pos = k->gen.source.find(placeholder, pos)) != std::string::npos;)
     k->gen.source.replace(pos, placeholder.size(), name);
   k->gen.name = name;
-  // the device function library is part of every translation unit: its text is part of the key, so a
-  // persisted cubin can never outlive the library it was compiled against
-  static const uint64_t lib_hash = Fnv1a(std::string(gdv_device_lib_text, static_cast<size_t>(gdv_device_lib_text_len)));
-  char lib_hex[24];
-  std::snprintf(lib_hex, sizeof(lib_hex), "%016llx", static_cast<unsigned long long>(lib_hash));
-  const std::string key = arch + (cfg.optimize ? "|O3|" : "|O0|") + (cfg.dump_ir ? "ptx|" : "|") + lib_hex + "|" + k->gen.source;
+  const std::string key = CubinKey(arch, cfg, k->gen.source);
   std::shared_ptr<const CachedCubin> hit;
   {
     std::lock_guard<std::mutex> lock(g_cache_mu);
     auto it = g_cubin_cache.find(key);
     if (it != g_cubin_cache.end()) hit = it->second;
   }
-  // GDV_CUBIN_CACHE_DIR=<dir>: cubins also persist across processes (the counterpart of the
-  // reference's object-code cache): <dir>/<fnv64 of arch|options|source>.cubin, written atomically.
-  std::string disk_path;
-  if (const char* cdir = std::getenv("GDV_CUBIN_CACHE_DIR")) {
-    if (!cfg.dump_ir) {  // DumpIR wants the PTX too: always compile
-      char kh[24];
-      std::snprintf(kh, sizeof(kh), "%016llx", static_cast<unsigned long long>(Fnv1a(key)));
-      disk_path = std::string(cdir) + "/" + kh + ".cubin";
-    }
-  }
+  const std::string disk_path = DiskCachePath(key, cfg);
   if (hit == nullptr && !disk_path.empty()) {
-    if (FILE* f = std::fopen(disk_path.c_str(), "rb")) {
-      std::vector<char> blob;
-      char buf[65536];
-      size_t got;
-      while ((got = std::fread(buf, 1, sizeof(buf), f)) > 0) blob.insert(blob.end(), buf, buf + got);
-      std::fclose(f);
-      const bool elf = blob.size() > 4 && blob[0] == 0x7f && blob[1] == 'E' && blob[2] == 'L' && blob[3] == 'F';
-      if (elf && std::search(blob.begin(), blob.end(), name.begin(), name.end()) != blob.end()) {
-        auto entry = std::make_shared<CachedCubin>();
-        entry->cubin = std::move(blob);
-        hit = entry;
-        std::lock_guard<std::mutex> lock(g_cache_mu);
-        if (g_cubin_cache.size() >= kCubinCacheEntries) g_cubin_cache.clear();
-        g_cubin_cache.emplace(key, entry);
-      }
-    }
+    hit = ReadDiskCubin(disk_path, name);
+    if (hit != nullptr) RememberCubin(key, hit);
   }
   if (hit != nullptr) {
     k->cubin = hit->cubin;
@@ -398,16 +445,7 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
     g_compile_count.fetch_add(1);
     GDV_RETURN_NOT_OK(CompileToCubin(k->gen.source, arch, cfg.optimize, cfg.dump_ir, &k->cubin,
                                      &k->ptx, &k->compile_log));
-    const bool elf_out = k->cubin.size() > 4 && k->cubin[0] == 0x7f && k->cubin[1] == 'E';
-    if (!disk_path.empty() && elf_out) {
-      const std::string tmp = disk_path + ".tmp" + std::to_string(static_cast<long long>(::getpid()));
-      if (FILE* f = std::fopen(tmp.c_str(), "wb")) {
-        const bool ok = std::fwrite(k->cubin.data(), 1, k->cubin.size(), f) == k->cubin.size();
-        std::fclose(f);
-        if (ok) std::rename(tmp.c_str(), disk_path.c_str());
-        else std::remove(tmp.c_str());
-      }
-    }
+    if (!disk_path.empty()) WriteDiskCubin(disk_path, k->cubin);
     // a translation unit can compile "successfully" without the kernel in it (e.g. when the
     // front end stops at a stray byte): make that a code-generation error here, not a missing
     // symbol at the first Evaluate on a GPU
@@ -417,46 +455,9 @@ Status BuildKernel(const Schema& schema, const std::vector<ExpressionPtr>& exprs
     entry->cubin = k->cubin;
     entry->ptx = k->ptx;
     entry->log = k->compile_log;
-    std::lock_guard<std::mutex> lock(g_cache_mu);
-    if (g_cubin_cache.size() >= kCubinCacheEntries) g_cubin_cache.clear();
-    g_cubin_cache.emplace(key, std::move(entry));
+    RememberCubin(key, std::move(entry));
   }
-  // GDV_DUMP_DIR=<dir>: write <kernel>.cu / <kernel>.cubin for offline SASS inspection
-  // (cuobjdump -sass) and so that ncu's source page can find the generated code, and <kernel>.info
-  // with the launch fields the fuser chose (one key=value per line), so that two versions of the
-  // fuser can be compared kernel by kernel.
-  if (const char* dir = std::getenv("GDV_DUMP_DIR")) {
-    const std::string base = std::string(dir) + "/" + k->gen.name;
-    if (FILE* f = std::fopen((base + ".cu").c_str(), "w")) {
-      std::fwrite(k->gen.source.data(), 1, k->gen.source.size(), f);
-      std::fclose(f);
-    }
-    if (FILE* f = std::fopen((base + ".info").c_str(), "w")) {
-      const GeneratedKernel& g = k->gen;
-      std::fprintf(f, "rows_per_thread=%d\nblock_threads=%d\nselection_mode=%d\nnullable=%d\n", g.rows_per_thread,
-                   g.block_threads, g.selection_mode, g.nullable ? 1 : 0);
-      for (size_t j = 0; j < g.inputs.size(); ++j) {
-        const gdv_type_t t = g.inputs[j].type.c();
-        std::fprintf(f, "input%zu=col %d type %d/%d/%d hoist %d\n", j, g.inputs[j].schema_index, t.id, t.precision,
-                     t.scale, g.inputs[j].hoist ? 1 : 0);
-      }
-      for (size_t o = 0; o < g.outputs.size(); ++o) {
-        const gdv_type_t t = g.outputs[o].c();
-        std::fprintf(f, "output%zu=type %d/%d/%d\n", o, t.id, t.precision, t.scale);
-      }
-      std::fprintf(f, "uses_ctx=%d\nin_bytes_per_row=%d\nout_bytes_per_row=%d\nargs_size=%zu\ndynamic_smem=%d\n",
-                   g.uses_ctx ? 1 : 0, g.in_bytes_per_row, g.out_bytes_per_row, g.args.size, g.dynamic_smem);
-      std::fprintf(f, "tile_rows=%lld\nkey_driven=%d\nstaged=%d\nstages=%d\ncta_tile_rows=%lld\n",
-                   static_cast<long long>(g.tile_rows), g.key_driven ? 1 : 0, g.staged ? 1 : 0, g.stages,
-                   static_cast<long long>(g.cta_tile_rows));
-      std::fprintf(f, "view_shortcuts=%d\ngated_stages=%d\n", g.view_shortcuts, g.gated_stages);
-      std::fclose(f);
-    }
-    if (FILE* f = std::fopen((base + ".cubin").c_str(), "wb")) {
-      std::fwrite(k->cubin.data(), 1, k->cubin.size(), f);
-      std::fclose(f);
-    }
-  }
+  if (const char* dir = std::getenv("GDV_DUMP_DIR")) DumpKernel(dir, *k);
   *out = std::move(k);
   return Status::OK();
 }
@@ -480,21 +481,37 @@ inline int64_t BitBytes(int64_t bit_begin, int64_t nbits) {
   return ((bit_begin & 7) + nbits + 7) / 8;
 }
 
+constexpr const char* kValuesMisaligned = "device values buffer of column %d is not aligned to its element width";
+constexpr const char* kIndicesMisaligned = "device indices buffer of column %d is not aligned to its element width";
+
+// A contiguous array of `bytes` bytes as the kernels read it.  A host array is staged into pooled scratch
+// with `pad` bytes to spare; a device array is read in place and must be aligned to `align` bytes, or the
+// call fails with `what` (a format that takes the column `col`).
+Status ResolveArray(Device* dev, const void* p, size_t bytes, size_t pad, size_t align, bool host, CUstream stream,
+                    ScratchScope* scratch, const char* what, int col, CUdeviceptr* out) {
+  if (host) {
+    GDV_RETURN_NOT_OK(scratch->Alloc(bytes + pad, out));
+    return bytes > 0 ? StagedHtoD(dev, *out, p, bytes, stream) : Status::OK();
+  }
+  if (reinterpret_cast<uintptr_t>(p) % align != 0) {
+    char msg[128];
+    std::snprintf(msg, sizeof(msg), what, col);
+    return Status::Make(GDV_INVALID, msg);
+  }
+  *out = reinterpret_cast<CUdeviceptr>(p);
+  return Status::OK();
+}
+
 // A bitmap of `nbits` bits from bit `off` on as the kernels read it: a 4-byte aligned word pointer
 // plus a bit shift in [0, 31] (host bitmaps are staged into pooled device memory first).
 Status ResolveBitmap(Device* dev, const void* bits, int64_t off, int64_t nbits, bool host, CUstream stream,
                      ScratchScope* scratch, CUdeviceptr* ptr, uint32_t* sh) {
   const uint8_t* p = static_cast<const uint8_t*>(bits) + (off >> 3);
   *sh = static_cast<uint32_t>(off & 7);
-  if (host) {
-    const size_t bytes = static_cast<size_t>(BitBytes(off, nbits));
-    GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 8, ptr));
-    if (bytes > 0) GDV_RETURN_NOT_OK(StagedHtoD(dev, *ptr, p, bytes, stream));
-  } else {
-    const uintptr_t mis = reinterpret_cast<uintptr_t>(p) & 3u;
-    *ptr = reinterpret_cast<CUdeviceptr>(p - mis);
-    *sh += static_cast<uint32_t>(8 * mis);
-  }
+  if (host) return ResolveArray(dev, p, static_cast<size_t>(BitBytes(off, nbits)), 8, 1, host, stream, scratch, nullptr, 0, ptr);
+  const uintptr_t mis = reinterpret_cast<uintptr_t>(p) & 3u;
+  *ptr = reinterpret_cast<CUdeviceptr>(p - mis);
+  *sh += static_cast<uint32_t>(8 * mis);
   return Status::OK();
 }
 
@@ -511,23 +528,18 @@ Status ResolveDictionary(Device* dev, int col, const gdv_column_t& c, bool host,
   const int32_t* offs = static_cast<const int32_t*>(dict->offsets) + dict->offset;
   if (dict->validity != nullptr)
     GDV_RETURN_NOT_OK(ResolveBitmap(dev, dict->validity, dict->offset, dict->length, host, stream, scratch, &r->dvl, &r->dvs));
+  GDV_RETURN_NOT_OK(ResolveArray(dev, offs, static_cast<size_t>(dict->length + 1) * 4, 0, 1, host, stream, scratch,
+                                 nullptr, col, &r->dof));
   if (!host) {
-    r->dof = reinterpret_cast<CUdeviceptr>(offs);
     r->var = reinterpret_cast<CUdeviceptr>(dict->data);
     return Status::OK();
   }
-  const size_t obytes = static_cast<size_t>(dict->length + 1) * 4;
-  GDV_RETURN_NOT_OK(scratch->Alloc(obytes, &r->dof));
-  GDV_RETURN_NOT_OK(StagedHtoD(dev, r->dof, offs, obytes, stream));
   const int64_t first = offs[0], last = offs[dict->length];
   if (first < 0 || last < first || (last > first && (dict->data == nullptr || last > dict->data_size)))
     return Status::Make(GDV_INVALID, what + ": the dictionary's offsets reach past its data buffer");
-  const size_t vbytes = static_cast<size_t>(last - first);
-  CUdeviceptr dv;
-  GDV_RETURN_NOT_OK(scratch->Alloc(vbytes + 16, &dv));
-  if (vbytes > 0)
-    GDV_RETURN_NOT_OK(StagedHtoD(dev, dv, static_cast<const uint8_t*>(dict->data) + first, vbytes, stream));
-  r->var = dv - static_cast<CUdeviceptr>(first);  // kernel addresses bytes as var + offs[i]
+  GDV_RETURN_NOT_OK(ResolveArray(dev, static_cast<const uint8_t*>(dict->data) + first, static_cast<size_t>(last - first),
+                                 16, 1, host, stream, scratch, nullptr, col, &r->var));
+  r->var -= static_cast<CUdeviceptr>(first);  // kernel addresses bytes as var + offs[i]
   return Status::OK();
 }
 
@@ -561,13 +573,11 @@ Status ResolveViewBuffers(Device* dev, int col, const gdv_column_t& c, bool host
     if (sz < 0) return Status::Make(GDV_INVALID, what + ": negative size of data buffer " + std::to_string(i));
     if (sz == 0) continue;
     if (vb->data[i] == nullptr) return Status::Make(GDV_INVALID, what + ": data buffer " + std::to_string(i) + " is null");
-    GDV_RETURN_NOT_OK(scratch->Alloc(static_cast<size_t>(sz) + 16, &table[static_cast<size_t>(i)]));
-    GDV_RETURN_NOT_OK(StagedHtoD(dev, table[static_cast<size_t>(i)], vb->data[i], static_cast<size_t>(sz), stream));
+    GDV_RETURN_NOT_OK(ResolveArray(dev, vb->data[i], static_cast<size_t>(sz), 16, 1, host, stream, scratch, nullptr, col,
+                                   &table[static_cast<size_t>(i)]));
   }
   GDV_RETURN_NOT_OK(StagedHtoD(dev, r->vbf, table.data(), tbytes, stream));
-  GDV_RETURN_NOT_OK(scratch->Alloc(tbytes, &r->vsz));
-  GDV_RETURN_NOT_OK(StagedHtoD(dev, r->vsz, vb->sizes, tbytes, stream));
-  return Status::OK();
+  return ResolveArray(dev, vb->sizes, tbytes, 0, 1, host, stream, scratch, nullptr, col, &r->vsz);
 }
 
 Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t* batch,
@@ -579,115 +589,47 @@ Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t*
     const ColumnSlot& slot = gen.inputs[j];
     if (slot.schema_index < 0 || slot.schema_index >= batch->num_columns)
       return Status::Make(GDV_INVALID, "batch has fewer columns than the schema");
-    const gdv_column_t& c = batch->columns[slot.schema_index];
+    const int col = slot.schema_index;
+    const gdv_column_t& c = batch->columns[col];
     ResolvedIn r;
     const int64_t off = c.offset;
     const DataType& t = slot.type;
     if (c.values == nullptr && n > 0)
-      return Status::Make(GDV_INVALID, "column " + std::to_string(slot.schema_index) +
-                                           " has no values buffer");
-    // ---- validity
-    // Bitmaps reach the kernel as a 4-byte aligned word pointer plus a bit shift in [0, 31].
-    if (c.validity != nullptr) {
-      const uint8_t* p = static_cast<const uint8_t*>(c.validity) + (off >> 3);
-      r.vsh = static_cast<uint32_t>(off & 7);
-      if (host) {
-        const size_t bytes = static_cast<size_t>(BitBytes(off, n));
-        CUdeviceptr dp;
-        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 8, &dp));
-        GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
-        r.vld = dp;
-      } else {
-        const uintptr_t mis = reinterpret_cast<uintptr_t>(p) & 3u;
-        r.vld = reinterpret_cast<CUdeviceptr>(p - mis);
-        r.vsh += static_cast<uint32_t>(8 * mis);
-      }
-    }
-    // ---- values
+      return Status::Make(GDV_INVALID, "column " + std::to_string(col) + " has no values buffer");
+    if (c.validity != nullptr)
+      GDV_RETURN_NOT_OK(ResolveBitmap(dev, c.validity, off, n, host, stream, scratch, &r.vld, &r.vsh));
+    const uint8_t* values = static_cast<const uint8_t*>(c.values);
     if (t.is_bool()) {
-      const uint8_t* p = static_cast<const uint8_t*>(c.values) + (off >> 3);
-      r.dsh = static_cast<uint32_t>(off & 7);
-      if (host) {
-        const size_t bytes = static_cast<size_t>(BitBytes(off, n));
-        CUdeviceptr dp;
-        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 8, &dp));
-        GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
-        r.val = dp;
-      } else {
-        const uintptr_t mis = reinterpret_cast<uintptr_t>(p) & 3u;
-        r.val = reinterpret_cast<CUdeviceptr>(p - mis);
-        r.dsh += static_cast<uint32_t>(8 * mis);
-      }
+      GDV_RETURN_NOT_OK(ResolveBitmap(dev, c.values, off, n, host, stream, scratch, &r.val, &r.dsh));
     } else if (t.is_dict()) {
       // the indices like a fixed-width column of the index type, then the dictionary
       const int w = DataType(t.index).width();
-      const uint8_t* p = static_cast<const uint8_t*>(c.values) + off * w;
-      if (host) {
-        const size_t bytes = static_cast<size_t>(n) * w;
-        CUdeviceptr dp;
-        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 16, &dp));
-        if (bytes > 0) GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
-        r.val = dp;
-      } else {
-        if (reinterpret_cast<uintptr_t>(p) % static_cast<uintptr_t>(w) != 0)
-          return Status::Make(GDV_INVALID, "device indices buffer of column " + std::to_string(slot.schema_index) +
-                                               " is not aligned to its element width");
-        r.val = reinterpret_cast<CUdeviceptr>(p);
-      }
-      GDV_RETURN_NOT_OK(ResolveDictionary(dev, slot.schema_index, c, host, stream, scratch, &r));
+      GDV_RETURN_NOT_OK(ResolveArray(dev, values + off * w, static_cast<size_t>(n) * w, 16, w, host, stream, scratch, kIndicesMisaligned, col,
+                                     &r.val));
+      GDV_RETURN_NOT_OK(ResolveDictionary(dev, col, c, host, stream, scratch, &r));
     } else if (t.is_view()) {
       // the 16-byte views like a fixed-width column, then the data buffers
-      const uint8_t* p = static_cast<const uint8_t*>(c.values) + off * 16;
-      if (host) {
-        const size_t bytes = static_cast<size_t>(n) * 16;
-        CUdeviceptr dp;
-        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 16, &dp));
-        if (bytes > 0) GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
-        r.val = dp;
-      } else {
-        if (reinterpret_cast<uintptr_t>(p) % 16u != 0)
-          return Status::Make(GDV_INVALID, "device views buffer of column " + std::to_string(slot.schema_index) +
-                                               " is not 16-byte aligned");
-        r.val = reinterpret_cast<CUdeviceptr>(p);
-      }
-      GDV_RETURN_NOT_OK(ResolveViewBuffers(dev, slot.schema_index, c, host, stream, scratch, &r));
+      GDV_RETURN_NOT_OK(ResolveArray(dev, values + off * 16, static_cast<size_t>(n) * 16, 16, 16, host, stream, scratch,
+                                     "device views buffer of column %d is not 16-byte aligned", col, &r.val));
+      GDV_RETURN_NOT_OK(ResolveViewBuffers(dev, col, c, host, stream, scratch, &r));
     } else if (t.is_varlen()) {
       const int32_t* offs = static_cast<const int32_t*>(c.values) + off;
+      GDV_RETURN_NOT_OK(ResolveArray(dev, offs, static_cast<size_t>(n + 1) * 4, 0, 1, host, stream, scratch, nullptr, col,
+                                     &r.val));
       if (host) {
-        const size_t obytes = static_cast<size_t>(n + 1) * 4;
-        CUdeviceptr dp;
-        GDV_RETURN_NOT_OK(scratch->Alloc(obytes, &dp));
-        GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, offs, obytes, stream));
-        r.val = dp;
         const int64_t first = n > 0 ? offs[0] : 0, last = n > 0 ? offs[n] : 0;
-        const size_t vbytes = static_cast<size_t>(last - first);
-        CUdeviceptr dv;
-        GDV_RETURN_NOT_OK(scratch->Alloc(vbytes + 16, &dv));
-        if (vbytes > 0)
-          GDV_RETURN_NOT_OK(StagedHtoD(dev, dv, static_cast<const uint8_t*>(c.var_data) + first, vbytes, stream));
-        // kernel addresses bytes as var + offs[r]; rebase so offs[0] lands on dv
-        r.var = dv - static_cast<CUdeviceptr>(first);
+        GDV_RETURN_NOT_OK(ResolveArray(dev, static_cast<const uint8_t*>(c.var_data) + first,
+                                       static_cast<size_t>(last - first), 16, 1, host, stream, scratch, nullptr, col,
+                                       &r.var));
+        // kernel addresses bytes as var + offs[r]; rebase so offs[0] lands on the staged bytes
+        r.var -= static_cast<CUdeviceptr>(first);
       } else {
-        r.val = reinterpret_cast<CUdeviceptr>(offs);
         r.var = reinterpret_cast<CUdeviceptr>(c.var_data);
       }
     } else {
       const int w = t.width();
-      const uint8_t* p = static_cast<const uint8_t*>(c.values) + off * w;
-      if (host) {
-        const size_t bytes = static_cast<size_t>(n) * w;
-        CUdeviceptr dp;
-        GDV_RETURN_NOT_OK(scratch->Alloc(bytes + 16, &dp));
-        if (bytes > 0)
-          GDV_RETURN_NOT_OK(StagedHtoD(dev, dp, p, bytes, stream));
-        r.val = dp;
-      } else {
-        if (reinterpret_cast<uintptr_t>(p) % static_cast<uintptr_t>(w) != 0)
-          return Status::Make(GDV_INVALID, "device values buffer of column " +
-                                               std::to_string(slot.schema_index) +
-                                               " is not aligned to its element width");
-        r.val = reinterpret_cast<CUdeviceptr>(p);
-      }
+      GDV_RETURN_NOT_OK(ResolveArray(dev, values + off * w, static_cast<size_t>(n) * w, 16, w, host, stream, scratch, kValuesMisaligned, col,
+                                     &r.val));
     }
     (*out)[j] = r;
   }
@@ -740,7 +682,82 @@ int SelWidth(int mode) {
   }
 }
 
+// Blocks for a grid-stride kernel: as many as the work needs, at most `blocks_per_sm` on each SM the
+// configuration leaves to the engine.
+unsigned GridFor(const Device* dev, const Config& cfg, int blocks_per_sm, int64_t blocks_needed) {
+  const int64_t cap = static_cast<int64_t>(std::max(1, dev->sm_count() - cfg.sm_reserve)) * blocks_per_sm;
+  return static_cast<unsigned>(std::min(blocks_needed, cap));
+}
+
+// The selection vector's `n` slots into `args` (host indices are staged into scratch), and where the
+// kernel reads the slot count when it stays on the device.
+Status PutSelection(Device* dev, const gdv_selection_t* sel, int64_t n, bool host, CUstream stream,
+                    ScratchScope* scratch, const ArgsLayout& L, std::vector<uint8_t>& args) {
+  CUdeviceptr dsel = 0;
+  GDV_RETURN_NOT_OK(ResolveArray(dev, sel->indices, static_cast<size_t>(n) * SelWidth(sel->mode), 16, 1, host, stream,
+                                 scratch, nullptr, 0, &dsel));
+  Put<CUdeviceptr>(args, L.off_sel, dsel);
+  if (sel->d_num_slots != nullptr) Put<CUdeviceptr>(args, L.off_n_ptr, reinterpret_cast<CUdeviceptr>(sel->d_num_slots));
+  return Status::OK();
+}
+
 }  // namespace
+
+// ======================================================================================
+// PendingTable
+// ======================================================================================
+Status PendingTable::Entry::ErrorBlock(Device* dev, CUstream stream, CUdeviceptr* out) {
+  if (d_err == 0) {
+    GDV_RETURN_NOT_OK(dev->Alloc(256, &d_err));
+    GDV_RETURN_NOT_OK(CuCheck(Driver().MemsetD8Async(d_err, 0, 256, stream), "memset err"));
+  }
+  *out = d_err;
+  return Status::OK();
+}
+
+Status PendingTable::Settle(Device* dev, CUstream stream, int64_t* num_slots) {
+  const DriverApi& d = Driver();
+  Entry pend;
+  bool have = false;
+  {
+    std::lock_guard<std::mutex> lock(mu_);
+    auto it = entries_.find(stream);
+    if (it != entries_.end()) {
+      pend = std::move(it->second);
+      entries_.erase(it);
+      have = true;
+    }
+  }
+  int err = 0;
+  uint64_t count = 0;
+  Status copy = Status::OK();
+  if (pend.d_err != 0) copy = CuCheck(d.MemcpyDtoHAsync(&err, pend.d_err, sizeof(int), stream), "D2H err");
+  if (copy.ok() && pend.d_count != 0)
+    copy = CuCheck(d.MemcpyDtoHAsync(&count, pend.d_count, sizeof(count), stream), "D2H count");
+  Status s = CuCheck(d.StreamSynchronize(stream), "cuStreamSynchronize");
+  std::string detail;  // a capacity error of a device-count string output: which output, how many bytes
+  if (copy.ok() && s.ok() && err == 3) {
+    for (const auto& vc : pend.var_checks) {
+      uint64_t total = 0;
+      if (d.MemcpyDtoHAsync(&total, vc.d_total, 8, stream) != CUDA_SUCCESS || d.StreamSynchronize(stream) != CUDA_SUCCESS) break;
+      if (total > static_cast<uint64_t>(vc.capacity)) {
+        detail = ": output " + std::to_string(vc.out_index) + " needs " + std::to_string(total) +
+                 " bytes, its var_capacity is " + std::to_string(vc.capacity);
+        break;
+      }
+    }
+  }
+  std::string user_text;
+  if (copy.ok() && s.ok() && err == kUserError) user_text = UserErrorText(pend.d_err, stream);
+  // on every path: the pending blocks go back to the pool once the stream is idle
+  if (pend.d_err != 0) dev->Free(pend.d_err);
+  for (auto p : pend.scratch) dev->Free(p);
+  GDV_RETURN_NOT_OK(copy);
+  GDV_RETURN_NOT_OK(s);
+  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, (err == kUserError ? user_text : ExecutionErrorMessage(err)) + detail);
+  if (num_slots != nullptr) *num_slots = have ? static_cast<int64_t>(count) : -1;
+  return Status::OK();
+}
 
 // ======================================================================================
 // Projector
@@ -808,10 +825,37 @@ Status Projector::BuildKernels() {
 
 // ---- consumers of a rope: temps first (gdv_rope_temps.h) ---------------------------------------------------
 namespace {
-SchemaPtr ExtendedSchema(const SchemaPtr& schema, const RopeTemps& rt) {
+// The first stage of the two-stage plan: the ropes that `exprs` consume become the expressions of `rt`,
+// `rewritten` reads them as columns of the returned schema, `schema` plus one column per temporary.
+SchemaPtr ExtractRopeTemps(const SchemaPtr& schema, const std::vector<ExpressionPtr>& exprs, RopeTemps* rt,
+                           std::vector<ExpressionPtr>* rewritten) {
+  for (const auto& e : exprs) {
+    NodePtr r;
+    ExtractRopes(e->root(), e->result().type.is_varlen(), rt, &r);
+    rewritten->push_back(std::make_shared<Expression>(r, e->result()));
+  }
   std::vector<Field> fields = schema->fields();
-  fields.insert(fields.end(), rt.fields.begin(), rt.fields.end());
+  fields.insert(fields.end(), rt->fields.begin(), rt->fields.end());
   return std::make_shared<Schema>(std::move(fields));
+}
+
+// Runs `eval` over `batch` extended by the temporaries `pre` materialises.  The temporaries of a device
+// batch go back to the pool when this returns: not before the work that reads them.
+template <typename Eval>
+Status EvaluateOverTemps(Projector* pre, const gdv_batch_t* batch, void* stream_v, Eval eval) {
+  TempColumns tc;
+  GDV_RETURN_NOT_OK(tc.Build(pre, batch, stream_v));
+  Status st = eval(&tc.batch);
+  if (batch->mem_space != GDV_MEM_HOST) {
+    Device* dev = nullptr;
+    Status w = Device::Get(pre->config().device, &dev);
+    if (w.ok()) {
+      CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
+      w = CuCheck(Driver().StreamSynchronize(stream), "cuStreamSynchronize");
+    }
+    if (st.ok()) st = w;
+  }
+  return st;
 }
 }  // namespace
 
@@ -819,11 +863,7 @@ Status Projector::MakeWithRopeTemps(const SchemaPtr& schema, const std::vector<E
                                     int selection_mode, const Config& cfg, Projector* into) {
   RopeTemps rt;
   std::vector<ExpressionPtr> rewritten;
-  for (const auto& e : exprs) {
-    NodePtr r;
-    ExtractRopes(e->root(), e->result().type.is_varlen(), &rt, &r);
-    rewritten.push_back(std::make_shared<Expression>(r, e->result()));
-  }
+  const SchemaPtr extended = ExtractRopeTemps(schema, exprs, &rt, &rewritten);
   if (rt.temps.empty()) return Status::Make(GDV_NOT_IMPLEMENTED, "no rope to materialise");
   // nesting: the temps' own Projector may need temporaries of its own (a consumer inside a rope's arguments)
   static thread_local int depth = 0;
@@ -835,7 +875,7 @@ Status Projector::MakeWithRopeTemps(const SchemaPtr& schema, const std::vector<E
   } level(depth);
   std::shared_ptr<Projector> pre, main;
   GDV_RETURN_NOT_OK(Projector::Make(schema, rt.temps, GDV_SEL_NONE, cfg, &pre));
-  GDV_RETURN_NOT_OK(Projector::Make(ExtendedSchema(schema, rt), rewritten, selection_mode, cfg, &main));
+  GDV_RETURN_NOT_OK(Projector::Make(extended, rewritten, selection_mode, cfg, &main));
   if (main->rope_main_ != nullptr) return Status::Make(GDV_NOT_IMPLEMENTED, "rope consumer left after materialisation");
   into->rope_pre_ = std::move(pre);
   into->rope_main_ = std::move(main);
@@ -910,16 +950,6 @@ Status TempColumns::Run(Projector* pre, const gdv_batch_t* eval, const gdv_batch
   batch.columns = cols.data();
   return Status::OK();
 }
-
-namespace {
-// The temps of a device batch go back to the pool when TempColumns dies: not before the work that reads them.
-Status WaitForStream(int device, void* stream_v) {
-  Device* dev = nullptr;
-  GDV_RETURN_NOT_OK(Device::Get(device, &dev));
-  CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
-  return CuCheck(Driver().StreamSynchronize(stream), "cuStreamSynchronize");
-}
-}  // namespace
 
 CompiledKernel& Projector::kernel() {
   if (rope_main_ != nullptr) return rope_main_->kernel();
@@ -1008,8 +1038,35 @@ Status Projector::CheckEvaluateArgs(const gdv_batch_t* batch, const gdv_selectio
   }
   *n = selection_mode_ != GDV_SEL_NONE ? sel->num_slots : batch->num_rows;
   if (*n < 0) return Status::Make(GDV_INVALID, "negative slot count");
+  if (selection_mode_ != GDV_SEL_NONE && sel->d_num_slots != nullptr && batch->mem_space == GDV_MEM_HOST)
+    return Status::Make(GDV_INVALID, "d_num_slots needs device buffers");
   return Status::OK();
 }
+
+namespace {
+Status CheckFilterArgs(const gdv_batch_t* batch, const gdv_selection_t* out_sel) {
+  if (batch->num_rows <= 0) return Status::Make(GDV_INVALID, "RecordBatch must be non-empty.");
+  // GDV_SEL_BOUNDED: the caller sized the index buffer for the rows it expects to be selected
+  // (row-range shards writing into a shared SelectionVector); rows past max_slots are counted
+  // but not stored, so count > max_slots tells the caller that the vector overflowed.
+  const bool bounded = (out_sel->mode & GDV_SEL_BOUNDED) != 0;
+  const int sel_mode = out_sel->mode & ~GDV_SEL_BOUNDED;
+  if (sel_mode < GDV_SEL_UINT16 || sel_mode > GDV_SEL_UINT64)
+    return Status::Make(GDV_INVALID, "invalid selection vector mode");
+  if (bounded && (batch->mem_space != GDV_MEM_DEVICE || out_sel->max_slots < 0))
+    return Status::Make(GDV_INVALID, "a bounded selection vector needs device buffers");
+  if (!bounded && out_sel->max_slots < batch->num_rows)
+    return Status::Make(GDV_INVALID, "Selection vector max_slots " + std::to_string(out_sel->max_slots) +
+                                         " is less than the number of rows " + std::to_string(batch->num_rows));
+  if (out_sel->mem_space != batch->mem_space)
+    return Status::Make(GDV_INVALID, "selection vector and batch must share a memory space");
+  if (sel_mode == GDV_SEL_UINT16 && batch->num_rows > 65536)
+    return Status::Make(GDV_INVALID, "batch too large for a uint16 selection vector");
+  if (sel_mode == GDV_SEL_UINT32 && batch->num_rows > (int64_t(1) << 32))
+    return Status::Make(GDV_INVALID, "batch too large for a uint32 selection vector");
+  return Status::OK();
+}
+}  // namespace
 
 // The two-stage rope plan sizes its temporaries on the host, synchronously, so it cannot take part in
 // a chain that keeps the slot count on the device: its utf8/binary outputs refuse d_num_slots.  (Its
@@ -1033,9 +1090,9 @@ Status Projector::OutputVarSize(const gdv_batch_t* batch, const gdv_selection_t*
     if (batch == nullptr) return Status::Make(GDV_INVALID, "null argument");
     for (const auto& sk : rope_main_->strings_)
       if (sk.out_index == out_index) GDV_RETURN_NOT_OK(RefuseDeviceCountWithRopeTemps(batch, sel));
-    TempColumns tc;
-    GDV_RETURN_NOT_OK(tc.Build(rope_pre_.get(), batch, stream));
-    return rope_main_->OutputVarSize(&tc.batch, sel, out_index, stream, bytes);  // synchronous: reads the total back
+    return EvaluateOverTemps(rope_pre_.get(), batch, stream, [&](const gdv_batch_t* with_temps) {
+      return rope_main_->OutputVarSize(with_temps, sel, out_index, stream, bytes);
+    });
   }
   for (auto& sk : strings_)
     if (sk.out_index == out_index)
@@ -1055,7 +1112,6 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   // passes and the scan read the count on the device, and the scan checks the total against the
   // caller's var_capacity (the host never sees the total before the write pass).
   const bool dev_count = selection_mode_ != GDV_SEL_NONE && sel->d_num_slots != nullptr;
-  if (dev_count && host) return Status::Make(GDV_INVALID, "d_num_slots needs device buffers");
   Device* dev = nullptr;
   GDV_RETURN_NOT_OK(Device::Get(cfg_.device, &dev));
   CompiledKernel *ksize = nullptr, *kwrite = nullptr;
@@ -1076,17 +1132,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
   PutInputs(args, L, ins);
-  if (selection_mode_ != GDV_SEL_NONE) {
-    CUdeviceptr dsel = reinterpret_cast<CUdeviceptr>(sel->indices);
-    if (host) {
-      const size_t bytes = static_cast<size_t>(n) * SelWidth(selection_mode_);
-      GDV_RETURN_NOT_OK(scratch.Alloc(bytes + 16, &dsel));
-      if (bytes > 0)
-        GDV_RETURN_NOT_OK(StagedHtoD(dev, dsel, sel->indices, bytes, stream));
-    }
-    Put<CUdeviceptr>(args, L.off_sel, dsel);
-    if (dev_count) Put<CUdeviceptr>(args, L.off_n_ptr, reinterpret_cast<CUdeviceptr>(sel->d_num_slots));
-  }
+  if (selection_mode_ != GDV_SEL_NONE) GDV_RETURN_NOT_OK(PutSelection(dev, sel, n, host, stream, &scratch, L, args));
   if (dev_count && !size_only) {
     if (out == nullptr || out->values == nullptr) return Status::Make(GDV_INVALID, "output offsets buffer is null");
     if (out->var_capacity < 0) return Status::Make(GDV_INVALID, "negative var_capacity");
@@ -1096,26 +1142,18 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   const int64_t n_tiles = (n + T - 1) / T;
   CUdeviceptr d_state = 0, d_err = 0;
   {
-    std::lock_guard<std::mutex> lock(mu_);
-    Pending& pend = pending_[stream];
-    pend.dev = dev;
+    auto pend = pending_.At(stream);
     GDV_RETURN_NOT_OK(dev->Alloc(16 + static_cast<size_t>(n_tiles) * 8, &d_state));
-    pend.scratch.push_back(d_state);
-    if (pend.d_err == 0) {
-      pend.uses_ctx = true;
-      GDV_RETURN_NOT_OK(dev->Alloc(256, &pend.d_err));
-      GDV_RETURN_NOT_OK(CuCheck(d.MemsetD8Async(pend.d_err, 0, 256, stream), "memset err"));
-    }
-    d_err = pend.d_err;
-    if (dev_count && !size_only) pend.var_checks.push_back({d_state, out->var_capacity, sk->out_index});
+    pend->scratch.push_back(d_state);
+    GDV_RETURN_NOT_OK(pend->ErrorBlock(dev, stream, &d_err));
+    if (dev_count && !size_only) pend->var_checks.push_back({d_state, out->var_capacity, sk->out_index});
   }
   Put<CUdeviceptr>(args, L.off_err, d_err);
   Put<CUdeviceptr>(args, L.off_tile_state, d_state + 16);
   Put<CUdeviceptr>(args, L.off_out_count, d_state);
-  const int64_t cap_blocks =
-      static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * lsize.blocks_per_sm;
-  unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap_blocks)));
-  GDV_RETURN_NOT_OK(LaunchKernel(dev, lsize, ksize->gen, args, grid, stream));
+  const int64_t blocks_needed = std::max<int64_t>(1, n_tiles);
+  GDV_RETURN_NOT_OK(LaunchKernel(dev, lsize, ksize->gen, args, GridFor(dev, cfg_, lsize.blocks_per_sm, blocks_needed),
+                                 stream));
   {
     CUfunction scan = nullptr;
     GDV_RETURN_NOT_OK(dev->StaticFunction("gdv_scan_tiles", &scan));
@@ -1169,10 +1207,8 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   Put<CUdeviceptr>(args, L.off_out_vld, d_vld);
   Put<CUdeviceptr>(args, L.off_out_var, d_data);
   Put<int64_t>(args, L.off_out_cap, out_cap);
-  const int64_t cap_w =
-      static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * lwrite.blocks_per_sm;
-  grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap_w)));
-  GDV_RETURN_NOT_OK(LaunchKernel(dev, lwrite, kwrite->gen, args, grid, stream));
+  GDV_RETURN_NOT_OK(LaunchKernel(dev, lwrite, kwrite->gen, args, GridFor(dev, cfg_, lwrite.blocks_per_sm, blocks_needed),
+                                 stream));
   if (host) {
     GDV_RETURN_NOT_OK(StagedDtoH(dev, out->values, d_offs, static_cast<size_t>(n + 1) * 4, stream));
     if (total > 0) GDV_RETURN_NOT_OK(StagedDtoH(dev, out->var_data, d_data, static_cast<size_t>(total), stream));
@@ -1194,14 +1230,9 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
     if (batch->num_columns != static_cast<int>(schema_->fields().size()))
       return Status::Make(GDV_INVALID, "RecordBatch schema must match the schema of Make()");
     if (!rope_main_->strings_.empty()) GDV_RETURN_NOT_OK(RefuseDeviceCountWithRopeTemps(batch, sel));
-    TempColumns tc;
-    GDV_RETURN_NOT_OK(tc.Build(rope_pre_.get(), batch, stream_v));
-    Status st = rope_main_->Evaluate(&tc.batch, sel, all_outs, n_all_outs, stream_v, async);
-    if (batch->mem_space != GDV_MEM_HOST) {
-      const Status w = WaitForStream(cfg_.device, stream_v);
-      if (st.ok()) st = w;
-    }
-    return st;
+    return EvaluateOverTemps(rope_pre_.get(), batch, stream_v, [&](const gdv_batch_t* with_temps) {
+      return rope_main_->Evaluate(with_temps, sel, all_outs, n_all_outs, stream_v, async);
+    });
   }
   int64_t n = 0;
   GDV_RETURN_NOT_OK(CheckEvaluateArgs(batch, sel, &n));
@@ -1228,7 +1259,6 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
   last_used_ = kernel;
   CompiledKernel::Loaded l;
   GDV_RETURN_NOT_OK(kernel->Load(dev, &l));
-  const DriverApi& d = Driver();
   CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
   const GeneratedKernel& gen = kernel->gen;
 
@@ -1243,21 +1273,7 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
   std::vector<uint8_t> args(L.size, 0);
   Put<int64_t>(args, L.off_n, n);
   PutInputs(args, L, ins);
-  // selection vector
-  if (selection_mode_ != GDV_SEL_NONE) {
-    CUdeviceptr dsel = reinterpret_cast<CUdeviceptr>(sel->indices);
-    if (host) {
-      const size_t bytes = static_cast<size_t>(n) * SelWidth(selection_mode_);
-      GDV_RETURN_NOT_OK(scratch.Alloc(bytes + 16, &dsel));
-      if (bytes > 0)
-        GDV_RETURN_NOT_OK(StagedHtoD(dev, dsel, sel->indices, bytes, stream));
-    }
-    Put<CUdeviceptr>(args, L.off_sel, dsel);
-    if (sel->d_num_slots != nullptr) {
-      if (host) return Status::Make(GDV_INVALID, "d_num_slots needs device buffers");
-      Put<CUdeviceptr>(args, L.off_n_ptr, reinterpret_cast<CUdeviceptr>(sel->d_num_slots));
-    }
-  }
+  if (selection_mode_ != GDV_SEL_NONE) GDV_RETURN_NOT_OK(PutSelection(dev, sel, n, host, stream, &scratch, L, args));
   // outputs
   struct OutStage {
     CUdeviceptr val = 0, vld = 0;
@@ -1282,28 +1298,16 @@ Status Projector::Evaluate(const gdv_batch_t* batch, const gdv_selection_t* sel,
     Put<CUdeviceptr>(args, L.off_out_val + 8 * o, st.val);
     Put<CUdeviceptr>(args, L.off_out_vld + 8 * o, st.vld);
   }
-  // error flag
-  CUdeviceptr d_err = 0;
   if (gen.uses_ctx) {
-    std::lock_guard<std::mutex> lock(mu_);
-    Pending& pend = pending_[stream];
-    if (pend.d_err == 0) {
-      pend.dev = dev;
-      pend.uses_ctx = true;
-      GDV_RETURN_NOT_OK(dev->Alloc(256, &pend.d_err));
-      GDV_RETURN_NOT_OK(CuCheck(d.MemsetD8Async(pend.d_err, 0, 256, stream), "memset err"));
-    }
-    d_err = pend.d_err;
+    CUdeviceptr d_err = 0;
+    GDV_RETURN_NOT_OK(pending_.At(stream)->ErrorBlock(dev, stream, &d_err));
     Put<CUdeviceptr>(args, L.off_err, d_err);
   }
 
   const int R = gen.rows_per_thread, BT = gen.block_threads;
   const int64_t wtiles = (n + 32 * R - 1) / (32 * R);
-  const int64_t blocks_needed = (wtiles + BT / 32 - 1) / (BT / 32);
-  const int64_t cap =
-      static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * l.blocks_per_sm;
-  const unsigned grid = static_cast<unsigned>(std::min<int64_t>(blocks_needed, cap));
-  GDV_RETURN_NOT_OK(LaunchKernel(dev, l, gen, args, grid, stream));
+  const int64_t blocks_needed = (wtiles + BT / 32 - 1) / (BT / 32);  // none for an empty selection
+  GDV_RETURN_NOT_OK(LaunchKernel(dev, l, gen, args, GridFor(dev, cfg_, l.blocks_per_sm, blocks_needed), stream));
 
   if (host) {
     const double t_launch = TraceOn() ? NowUs() : 0.0;
@@ -1330,45 +1334,7 @@ Status Projector::Sync(void* stream_v) {
   if (rope_main_ != nullptr) return rope_main_->Sync(stream_v);
   Device* dev = nullptr;
   GDV_RETURN_NOT_OK(Device::Get(cfg_.device, &dev));
-  CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
-  const DriverApi& d = Driver();
-  Pending pend;
-  bool have = false;
-  {
-    std::lock_guard<std::mutex> lock(mu_);
-    auto it = pending_.find(stream);
-    if (it != pending_.end()) {
-      pend = it->second;
-      pending_.erase(it);
-      have = true;
-    }
-  }
-  int err = 0;
-  Status copy = Status::OK();
-  if (have && pend.d_err != 0) copy = CuCheck(d.MemcpyDtoHAsync(&err, pend.d_err, sizeof(int), stream), "D2H err");
-  Status s = CuCheck(d.StreamSynchronize(stream), "cuStreamSynchronize");
-  std::string detail;  // a capacity error of a device-count string output: which output, how many bytes
-  if (copy.ok() && s.ok() && err == 3) {
-    for (const auto& vc : pend.var_checks) {
-      uint64_t total = 0;
-      if (d.MemcpyDtoHAsync(&total, vc.d_total, 8, stream) != CUDA_SUCCESS || d.StreamSynchronize(stream) != CUDA_SUCCESS) break;
-      if (total > static_cast<uint64_t>(vc.capacity)) {
-        detail = ": output " + std::to_string(vc.out_index) + " needs " + std::to_string(total) +
-                 " bytes, its var_capacity is " + std::to_string(vc.capacity);
-        break;
-      }
-    }
-  }
-  std::string user_text;
-  if (copy.ok() && s.ok() && err == kUserError) user_text = UserErrorText(pend.d_err, stream);
-  if (have) {  // on every path: the pending blocks go back to the pool once the stream is idle
-    if (pend.d_err != 0) dev->Free(pend.d_err);
-    for (auto p : pend.scratch) dev->Free(p);
-  }
-  GDV_RETURN_NOT_OK(copy);
-  GDV_RETURN_NOT_OK(s);
-  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, (err == kUserError ? user_text : ExecutionErrorMessage(err)) + detail);
-  return Status::OK();
+  return pending_.Settle(dev, stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream(), nullptr);
 }
 
 // ======================================================================================
@@ -1392,13 +1358,14 @@ Status Filter::Make(SchemaPtr schema, ConditionPtr cond, const Config& cfg,
     if (!IsRopeConsumerError(st)) return st;
     // something in the condition reads a rope: materialise the ropes first (gdv_rope_temps.h)
     RopeTemps rt;
-    NodePtr r;
-    ExtractRopes(cond->root(), false, &rt, &r);
+    std::vector<ExpressionPtr> rewritten;
+    const SchemaPtr extended = ExtractRopeTemps(schema, {cond}, &rt, &rewritten);
     if (rt.temps.empty()) return st;
     std::shared_ptr<Projector> pre;
     std::shared_ptr<Filter> main;
     Status two_stage = Projector::Make(schema, rt.temps, GDV_SEL_NONE, cfg, &pre);
-    if (two_stage.ok()) two_stage = Filter::Make(ExtendedSchema(schema, rt), std::make_shared<Condition>(r), cfg, &main);
+    if (two_stage.ok())
+      two_stage = Filter::Make(extended, std::make_shared<Condition>(rewritten[0]->root()), cfg, &main);
     if (two_stage.ok() && main->rope_main_ != nullptr) two_stage = st;
     if (!two_stage.ok()) return IsRopeConsumerError(two_stage) ? st : two_stage;  // another limit of the fuser: say that one
     f->rope_pre_ = std::move(pre);
@@ -1460,19 +1427,11 @@ Status Filter::LaunchDictionaryFirst(Device* dev, const gdv_batch_t* batch, CUst
   // 2. the rows: indices and their validity only
   const DataType it(schema_->fields()[static_cast<size_t>(dict_column_)].type.index);
   const int w = it.width();
-  const uint8_t* p = static_cast<const uint8_t*>(c.values) + c.offset * w;
   if (c.values == nullptr) return Status::Make(GDV_INVALID, "dictionary column has no indices buffer");
   CUdeviceptr d_in = 0, d_vld = 0;
   uint32_t vsh = 0;
-  if (host) {
-    GDV_RETURN_NOT_OK(scratch->Alloc(static_cast<size_t>(n) * w + 16, &d_in));
-    GDV_RETURN_NOT_OK(StagedHtoD(dev, d_in, p, static_cast<size_t>(n) * w, stream));
-  } else {
-    if (reinterpret_cast<uintptr_t>(p) % static_cast<uintptr_t>(w) != 0)
-      return Status::Make(GDV_INVALID, "device indices buffer of column " + std::to_string(dict_column_) +
-                                           " is not aligned to its element width");
-    d_in = reinterpret_cast<CUdeviceptr>(p);
-  }
+  GDV_RETURN_NOT_OK(ResolveArray(dev, static_cast<const uint8_t*>(c.values) + c.offset * w, static_cast<size_t>(n) * w,
+                                 16, w, host, stream, scratch, kIndicesMisaligned, dict_column_, &d_in));
   if (c.validity != nullptr)
     GDV_RETURN_NOT_OK(ResolveBitmap(dev, c.validity, c.offset, n, host, stream, scratch, &d_vld, &vsh));
   const std::string name = std::string("gdv_dict_filter_") + it.ctype() + (large ? "_w4" : "_w1");
@@ -1484,8 +1443,7 @@ Status Filter::LaunchDictionaryFirst(Device* dev, const gdv_batch_t* batch, CUst
   const DriverApi& d = Driver();
   int per_sm = 1;
   if (d.OccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, smem) != CUDA_SUCCESS || per_sm < 1) per_sm = 1;
-  const int64_t cap = static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * per_sm;
-  const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap)));
+  const unsigned grid = GridFor(dev, cfg_, per_sm, std::max<int64_t>(1, n_tiles));
   CUdeviceptr tile_state = d_state + 16, ticket = d_state;
   int64_t nn = n, rb = row_base, oc = out_cap, dl = dlen;
   int ow = idx_width;
@@ -1529,37 +1487,14 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
   if (batch->num_columns != static_cast<int>(schema_->fields().size()))
     return Status::Make(GDV_INVALID, "RecordBatch schema must match the schema of Make()");
   if (rope_main_ != nullptr) {
-    TempColumns tc;
-    GDV_RETURN_NOT_OK(tc.Build(rope_pre_.get(), batch, stream_v));
-    Status st = rope_main_->Evaluate(&tc.batch, out_sel, stream_v, async, d_count_user);
-    if (batch->mem_space != GDV_MEM_HOST) {
-      const Status w = WaitForStream(cfg_.device, stream_v);
-      if (st.ok()) st = w;
-    }
-    return st;
+    return EvaluateOverTemps(rope_pre_.get(), batch, stream_v, [&](const gdv_batch_t* with_temps) {
+      return rope_main_->Evaluate(with_temps, out_sel, stream_v, async, d_count_user);
+    });
   }
-  if (batch->num_rows <= 0) return Status::Make(GDV_INVALID, "RecordBatch must be non-empty.");
-  // GDV_SEL_BOUNDED: the caller sized the index buffer for the rows it expects to be selected
-  // (row-range shards writing into a shared SelectionVector); rows past max_slots are counted
-  // but not stored, so count > max_slots tells the caller that the vector overflowed.
+  GDV_RETURN_NOT_OK(CheckFilterArgs(batch, out_sel));
   const bool bounded = (out_sel->mode & GDV_SEL_BOUNDED) != 0;
   const int sel_mode = out_sel->mode & ~GDV_SEL_BOUNDED;
-  if (sel_mode < GDV_SEL_UINT16 || sel_mode > GDV_SEL_UINT64)
-    return Status::Make(GDV_INVALID, "invalid selection vector mode");
-  if (bounded && (batch->mem_space != GDV_MEM_DEVICE || out_sel->max_slots < 0))
-    return Status::Make(GDV_INVALID, "a bounded selection vector needs device buffers");
-  if (!bounded && out_sel->max_slots < batch->num_rows)
-    return Status::Make(GDV_INVALID, "Selection vector max_slots " +
-                                         std::to_string(out_sel->max_slots) +
-                                         " is less than the number of rows " +
-                                         std::to_string(batch->num_rows));
-  if (out_sel->mem_space != batch->mem_space)
-    return Status::Make(GDV_INVALID, "selection vector and batch must share a memory space");
   const int64_t n = batch->num_rows;
-  if (sel_mode == GDV_SEL_UINT16 && n > 65536)
-    return Status::Make(GDV_INVALID, "batch too large for a uint16 selection vector");
-  if (sel_mode == GDV_SEL_UINT32 && n > (int64_t(1) << 32))
-    return Status::Make(GDV_INVALID, "batch too large for a uint32 selection vector");
   const bool host = batch->mem_space == GDV_MEM_HOST;
 
   Device* dev = nullptr;
@@ -1593,37 +1528,27 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
   const size_t state_bytes = 16 + static_cast<size_t>(n_tiles) * 8;
   CUdeviceptr d_state = 0, d_err = 0, d_bits = 0;
   {
-    std::lock_guard<std::mutex> lock(mu_);
-    Pending& pend = pending_[stream];
-    pend.dev = dev;
-    if (pend.state_cap < state_bytes) {
+    auto pend = pending_.At(stream);
+    if (pend->state_cap < state_bytes) {
       // earlier blocks stay alive until Sync(): launches still queued may be using them
-      GDV_RETURN_NOT_OK(dev->Alloc(state_bytes, &pend.d_state));
-      pend.scratch.push_back(pend.d_state);
-      pend.state_cap = state_bytes;
+      GDV_RETURN_NOT_OK(dev->Alloc(state_bytes, &pend->d_state));
+      pend->scratch.push_back(pend->d_state);
+      pend->state_cap = state_bytes;
     }
-    d_state = pend.d_state;
+    d_state = pend->d_state;
     if (dict_first) {
       const auto* dict = static_cast<const gdv_dictionary_t*>(batch->columns[dict_column_].var_data);
       const int64_t dlen = dict != nullptr ? dict->length : 0;
       const size_t bits_bytes = static_cast<size_t>(std::max<int64_t>(dlen, 0) + 31) / 32 * 4 + 16;
-      if (pend.bits_cap < bits_bytes) {
-        GDV_RETURN_NOT_OK(dev->Alloc(bits_bytes, &pend.d_bits));
-        pend.scratch.push_back(pend.d_bits);
-        pend.bits_cap = bits_bytes;
+      if (pend->bits_cap < bits_bytes) {
+        GDV_RETURN_NOT_OK(dev->Alloc(bits_bytes, &pend->d_bits));
+        pend->scratch.push_back(pend->d_bits);
+        pend->bits_cap = bits_bytes;
       }
-      d_bits = pend.d_bits;
+      d_bits = pend->d_bits;
     }
-    if (!dict_first && kernel->gen.uses_ctx) {
-      if (pend.d_err == 0) {
-        GDV_RETURN_NOT_OK(dev->Alloc(256, &pend.d_err));
-        GDV_RETURN_NOT_OK(CuCheck(d.MemsetD8Async(pend.d_err, 0, 256, stream), "memset err"));
-        pend.uses_ctx = true;
-      }
-      d_err = pend.d_err;
-    }
-    pend.d_count = d_count_user != nullptr ? reinterpret_cast<CUdeviceptr>(d_count_user)
-                                           : d_state + 8;
+    if (!dict_first && kernel->gen.uses_ctx) GDV_RETURN_NOT_OK(pend->ErrorBlock(dev, stream, &d_err));
+    pend->d_count = d_count_user != nullptr ? reinterpret_cast<CUdeviceptr>(d_count_user) : d_state + 8;
   }
   GDV_RETURN_NOT_OK(CuCheck(d.MemsetD8Async(d_state, 0, state_bytes, stream), "memset tile state"));
   CUdeviceptr d_count = d_state + 8;
@@ -1652,10 +1577,8 @@ Status Filter::Evaluate(const gdv_batch_t* batch, gdv_selection_t* out_sel, void
     Put<CUdeviceptr>(args, L.off_err, d_err);
     Put<int64_t>(args, L.off_out_cap, bounded ? out_sel->max_slots : n);
     PutInputs(args, L, ins);
-    const int64_t cap =
-        static_cast<int64_t>(std::max(1, dev->sm_count() - cfg_.sm_reserve)) * l.blocks_per_sm;
-    const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(n_tiles, cap)));
-    GDV_RETURN_NOT_OK(LaunchKernel(dev, l, gen, args, grid, stream));
+    GDV_RETURN_NOT_OK(LaunchKernel(dev, l, gen, args, GridFor(dev, cfg_, l.blocks_per_sm, std::max<int64_t>(1, n_tiles)),
+                                   stream));
   }
 
   out_sel->num_slots = -1;
@@ -1681,37 +1604,7 @@ Status Filter::Sync(void* stream_v, int64_t* num_slots) {
   if (rope_main_ != nullptr) return rope_main_->Sync(stream_v, num_slots);
   Device* dev = nullptr;
   GDV_RETURN_NOT_OK(Device::Get(cfg_.device, &dev));
-  CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
-  const DriverApi& d = Driver();
-  Pending pend;
-  bool have = false;
-  {
-    std::lock_guard<std::mutex> lock(mu_);
-    auto it = pending_.find(stream);
-    if (it != pending_.end()) {
-      pend = it->second;
-      pending_.erase(it);
-      have = true;
-    }
-  }
-  int err = 0;
-  uint64_t count = 0;
-  Status copy = Status::OK();
-  if (have && pend.d_err != 0) copy = CuCheck(d.MemcpyDtoHAsync(&err, pend.d_err, sizeof(int), stream), "D2H err");
-  if (copy.ok() && have && pend.d_count != 0)
-    copy = CuCheck(d.MemcpyDtoHAsync(&count, pend.d_count, sizeof(count), stream), "D2H count");
-  Status s = CuCheck(d.StreamSynchronize(stream), "cuStreamSynchronize");
-  std::string user_text;
-  if (copy.ok() && s.ok() && err == kUserError) user_text = UserErrorText(pend.d_err, stream);
-  if (have) {  // on every path: the pending blocks go back to the pool once the stream is idle
-    if (pend.d_err != 0) dev->Free(pend.d_err);
-    for (auto p : pend.scratch) dev->Free(p);
-  }
-  GDV_RETURN_NOT_OK(copy);
-  GDV_RETURN_NOT_OK(s);
-  if (err != 0) return Status::Make(GDV_EXECUTION_ERROR, err == kUserError ? user_text : ExecutionErrorMessage(err));
-  if (num_slots != nullptr) *num_slots = have ? static_cast<int64_t>(count) : -1;
-  return Status::OK();
+  return pending_.Settle(dev, stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream(), num_slots);
 }
 
 }  // namespace gdv

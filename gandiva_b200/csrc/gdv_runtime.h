@@ -34,7 +34,6 @@ class Device {
   // stream-ordered scratch or error / count read-backs.  The thread that created the Device uses
   // stream_; other threads get theirs on first use (destroyed when the thread exits).
   CUstream stream() const;
-  CUstream copy_stream() const { return copy_stream_; }
 
   // Pooled device scratch: freed blocks are cached and reused (no cuMemFree on the hot path).  The
   // cache is bounded: once the idle blocks hold more than the limit (default 4 GiB, GDV_POOL_LIMIT_MB
@@ -56,7 +55,6 @@ class Device {
   CUdevice dev_ = 0;
   CUcontext ctx_ = nullptr;
   CUstream stream_ = nullptr;
-  CUstream copy_stream_ = nullptr;
   std::thread::id owner_thread_;
   int sm_count_ = 0, cc_major_ = 0, cc_minor_ = 0;
   std::mutex mu_;
@@ -92,13 +90,11 @@ class ScratchScope {
   explicit ScratchScope(Device* d) : dev_(d) {}
   // Work that reads or writes the blocks may still be queued on `stream` when an Evaluate returns
   // early with an error: the destructor then waits for the stream before the blocks go back to the
-  // pool (where another thread could be handed them).  Settled() after the call's own final
-  // synchronisation skips that wait.
+  // pool (where another thread could be handed them).
   void Guard(CUstream stream) {
     stream_ = stream;
     guarded_ = true;
   }
-  void Settled() { guarded_ = false; }
   ~ScratchScope() {
     if (guarded_ && !blocks_.empty()) Driver().StreamSynchronize(stream_);
     for (auto p : blocks_) dev_->Free(p);
@@ -107,11 +103,6 @@ class ScratchScope {
     Status s = dev_->Alloc(bytes, out);
     if (s.ok()) blocks_.push_back(*out);
     return s;
-  }
-  std::vector<CUdeviceptr> Release() {
-    std::vector<CUdeviceptr> b;
-    b.swap(blocks_);
-    return b;
   }
 
  private:
@@ -160,25 +151,48 @@ class CompiledKernel {
   std::map<int, Loaded> loaded_;
 };
 
-// Pending asynchronous evaluation state (error flag / count readback) per stream.
-struct Pending {
-  Device* dev = nullptr;
-  std::vector<CUdeviceptr> scratch;  // returned to the pool at sync
-  CUdeviceptr d_err = 0;
-  CUdeviceptr d_count = 0;
-  CUdeviceptr d_state = 0;  // filter look-back state, reused by stream-ordered launches
-  size_t state_cap = 0;
-  CUdeviceptr d_bits = 0;   // dictionary-first filter: one bit per dictionary entry
-  size_t bits_cap = 0;
-  bool uses_ctx = false;
-  // projector, utf8/binary outputs with a device slot count: where each scan left its byte total,
-  // the output's var_capacity and index (they name the output a capacity error is about)
-  struct VarCheck {
-    CUdeviceptr d_total;
-    int64_t capacity;
-    int out_index;
+// What asynchronous evaluations on each stream leave for its Sync: the error block, the count to read
+// back and the scratch blocks the queued work uses.
+class PendingTable {
+ public:
+  struct Entry {
+    std::vector<CUdeviceptr> scratch;  // returned to the pool at Settle
+    CUdeviceptr d_err = 0;
+    CUdeviceptr d_count = 0;
+    CUdeviceptr d_state = 0;  // filter look-back state, reused by stream-ordered launches
+    size_t state_cap = 0;
+    CUdeviceptr d_bits = 0;   // dictionary-first filter: one bit per dictionary entry
+    size_t bits_cap = 0;
+    // projector, utf8/binary outputs with a device slot count: where each scan left its byte total,
+    // the output's var_capacity and index (they name the output a capacity error is about)
+    struct VarCheck {
+      CUdeviceptr d_total;
+      int64_t capacity;
+      int out_index;
+    };
+    std::vector<VarCheck> var_checks;
+    // The stream's 256-byte error block: allocated and zeroed on the stream by its first user.
+    Status ErrorBlock(Device* dev, CUstream stream, CUdeviceptr* out);
   };
-  std::vector<VarCheck> var_checks;
+  // The stream's entry, with the table locked while the handle lives.
+  struct Locked {
+    std::unique_lock<std::mutex> lock;
+    Entry* entry;
+    Entry* operator->() const { return entry; }
+  };
+  Locked At(CUstream stream) {
+    std::unique_lock<std::mutex> lock(mu_);
+    Entry* e = &entries_[stream];
+    return {std::move(lock), e};
+  }
+  // Takes the stream's entry out, reads its error word (and its count, when one was registered) back,
+  // waits for the stream and returns the entry's blocks to the pool on every path.  *count: the count,
+  // or -1 when nothing was pending.
+  Status Settle(Device* dev, CUstream stream, int64_t* count);
+
+ private:
+  std::mutex mu_;
+  std::map<void*, Entry> entries_;
 };
 
 class Projector {
@@ -233,8 +247,8 @@ class Projector {
   std::unique_ptr<CompiledKernel> kernel_;          // general (nullable) variant, built at Make()
   std::unique_ptr<CompiledKernel> kernel_nonull_;   // built on first batch without nulls
   std::atomic<CompiledKernel*> last_used_{nullptr};  // variant of the latest Evaluate (kernel_info)
-  std::mutex mu_;
-  std::map<void*, Pending> pending_;
+  std::mutex mu_;  // guards the lazily built kernels; never held with pending_'s lock
+  PendingTable pending_;
 };
 
 class Filter {
@@ -271,9 +285,9 @@ class Filter {
   SchemaPtr schema_;
   ConditionPtr cond_;
   Config cfg_;
-  mutable std::mutex mu_;
+  mutable std::mutex mu_;  // guards kernels_; never held with pending_'s lock
   std::map<int, std::unique_ptr<CompiledKernel>> kernels_;
-  std::map<void*, Pending> pending_;
+  PendingTable pending_;
 };
 
 const char* ExecutionErrorMessage(int code);
