@@ -239,6 +239,8 @@ GDV_TYPE_DICTIONARY = 29
 GDV_DICT_ORDERED = 0x100
 GDV_TYPE_STRING_VIEW = 39
 GDV_TYPE_BINARY_VIEW = 40
+GDV_TYPE_LARGE_STRING = 34
+GDV_TYPE_LARGE_BINARY = 35
 
 
 def _to_c_type(t: pa.DataType) -> gdv_type_t:
@@ -257,7 +259,8 @@ def _from_c_type(t: gdv_type_t) -> pa.DataType:
     simple = {1: pa.bool_(), 2: pa.uint8(), 3: pa.int8(), 4: pa.uint16(), 5: pa.int16(),
               6: pa.uint32(), 7: pa.int32(), 8: pa.uint64(), 9: pa.int64(), 11: pa.float32(),
               12: pa.float64(), 13: pa.string(), 14: pa.binary(), 16: pa.date32(),
-              17: pa.date64(), GDV_TYPE_STRING_VIEW: pa.string_view(), GDV_TYPE_BINARY_VIEW: pa.binary_view()}
+              17: pa.date64(), GDV_TYPE_STRING_VIEW: pa.string_view(), GDV_TYPE_BINARY_VIEW: pa.binary_view(),
+              GDV_TYPE_LARGE_STRING: pa.large_string(), GDV_TYPE_LARGE_BINARY: pa.large_binary()}
     if tid in simple:
         return simple[tid]
     if tid == GDV_TYPE_DICTIONARY:
@@ -404,7 +407,7 @@ class TreeExprBuilder:
             if isinstance(value, (str, bytes)):
                 raise TypeError("float literal expected")
             raw = np.array([value], dtype=np.float32 if pa.types.is_float32(t) else np.float64).tobytes()
-        elif pa.types.is_string(t) or pa.types.is_binary(t):
+        elif _is_varlen(t):
             if isinstance(value, str):
                 raw = value.encode("utf-8")
             elif isinstance(value, (bytes, bytearray)):
@@ -482,7 +485,7 @@ class TreeExprBuilder:
         t = _ensure_type(dtype)
         values = list(values)
         out = C.c_void_p()
-        if pa.types.is_string(t) or pa.types.is_binary(t):
+        if _is_varlen(t):
             raws = [v.encode("utf-8") if isinstance(v, str) else bytes(v) for v in values]
             blob = b"".join(raws)
             lens = (C.c_int32 * max(len(raws), 1))(*[len(r) for r in raws])
@@ -630,6 +633,11 @@ def _view_buffers_to_c(arr: pa.Array) -> gdv_view_buffers_t:
     return c
 
 
+def _is_varlen(t: pa.DataType) -> bool:
+    """utf8 / binary with contiguous bytes behind int32 or int64 offsets."""
+    return pa.types.is_string(t) or pa.types.is_binary(t) or pa.types.is_large_string(t) or pa.types.is_large_binary(t)
+
+
 def _batch_to_c(batch: pa.RecordBatch):
     """RecordBatch -> gdv_batch_t over the batch's own buffers (no copies)."""
     cols = (gdv_column_t * max(batch.num_columns, 1))()
@@ -654,7 +662,8 @@ def _batch_to_c(batch: pa.RecordBatch):
             v = _view_buffers_to_c(arr)
             keep.append(v)
             c.var_data = C.addressof(v)
-        elif pa.types.is_string(t) or pa.types.is_binary(t):
+        elif _is_varlen(t):
+            # int32 offsets, or int64 for large_string / large_binary; var_data -> the bytes
             c.values = bufs[1].address if bufs[1] is not None else None
             c.var_data = bufs[2].address if len(bufs) > 2 and bufs[2] is not None else None
             c.var_data_size = bufs[2].size if len(bufs) > 2 and bufs[2] is not None else 0
@@ -760,11 +769,12 @@ class Projector:
             vbytes = (n + 7) // 8
             vbuf = np.zeros((vbytes + 7) // 8 * 8, dtype=np.uint8)
             var = None
-            if pa.types.is_string(t) or pa.types.is_binary(t):
+            if _is_varlen(t):
                 # utf8/binary: size the data buffer with the sizing pass, as the C++ layer does
                 need = C.c_int64(0)
                 _check(lib.gdv_projector_output_var_size(self._h, C.byref(cb), csel, i, None, C.byref(need)))
-                dbuf = np.zeros(n + 1, dtype=np.int32)
+                large = pa.types.is_large_string(t) or pa.types.is_large_binary(t)
+                dbuf = np.zeros(n + 1, dtype=np.int64 if large else np.int32)
                 var = np.zeros(max(need.value, 8), dtype=np.uint8)
                 outs[i].var_data = var.ctypes.data_as(C.c_void_p)
                 outs[i].var_capacity = need.value
@@ -791,9 +801,10 @@ class Projector:
         """columns: per schema field (validity_ptr|0, values_ptr, var_data_ptr|0, offset), where a
         dictionary-encoded column passes its indices as values and a gdv_dictionary_t as var_data, and
         a string_view / binary_view column its 16-byte views and a gdv_view_buffers_t (view_buffers());
+        a large_string / large_binary column passes its int64 offsets as values and its bytes as var_data;
         outputs: per expression (validity_ptr|0, values_ptr), or for a utf8 / binary output
         (validity_ptr|0, offsets_ptr, var_data_ptr, var_capacity) with room for num_slots + 1 int32
-        offsets; selection: (ptr, num_slots) or (ptr, max_slots, d_count_ptr): the slot count is read
+        offsets (int64 for a large_string / large_binary output); selection: (ptr, num_slots) or (ptr, max_slots, d_count_ptr): the slot count is read
         from device memory (the d_count a Filter.evaluate_device(..., sync=False) wrote on the same
         stream), no host round trip.  A utf8 / binary output whose bytes exceed its var_capacity raises
         ExecutionError here (sync=True) or from sync().  With sync=True returns each output's var_size

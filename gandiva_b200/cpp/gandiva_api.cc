@@ -66,6 +66,8 @@ DataTypePtr FromC(const gdv_type_t& t) {
     case GDV_TYPE_BINARY: return arrow::binary();
     case GDV_TYPE_STRING_VIEW: return arrow::utf8_view();
     case GDV_TYPE_BINARY_VIEW: return arrow::binary_view();
+    case GDV_TYPE_LARGE_STRING: return arrow::large_utf8();
+    case GDV_TYPE_LARGE_BINARY: return arrow::large_binary();
     case GDV_TYPE_DATE32: return arrow::date32();
     case GDV_TYPE_DATE64: return arrow::date64();
     case GDV_TYPE_TIMESTAMP: return arrow::timestamp(static_cast<arrow::TimeUnit::type>(t.precision));
@@ -622,13 +624,14 @@ Status Projector::Evaluate(const arrow::RecordBatch& batch, const SelectionVecto
     const int64_t bitmap_bytes = arrow::bit_util::RoundUpToMultipleOf8(arrow::bit_util::BytesForBits(n)) + 8;
     ARROW_ASSIGN_OR_RAISE(std::shared_ptr<arrow::Buffer> validity, alloc(bitmap_bytes, true));
     outs[i].validity = reinterpret_cast<void*>(validity->address());
-    if (t->id() == arrow::Type::STRING || t->id() == arrow::Type::BINARY) {
+    const bool large = t->id() == arrow::Type::LARGE_STRING || t->id() == arrow::Type::LARGE_BINARY;
+    if (t->id() == arrow::Type::STRING || t->id() == arrow::Type::BINARY || large) {
       // utf8/binary: the sizing pass says how many bytes the data buffer needs, then the
-      // offsets (n + 1 int32) and the bytes are allocated
+      // offsets (n + 1 int32, or int64 for large_string / large_binary) and the bytes are allocated
       int64_t need = 0;
       ARROW_RETURN_NOT_OK(ToStatus(gdv_projector_output_var_size(
           static_cast<gdv_projector_t>(handle_), &b, psel, static_cast<int32_t>(i), nullptr, &need)));
-      ARROW_ASSIGN_OR_RAISE(std::shared_ptr<arrow::Buffer> offsets, alloc((n + 1) * 4 + 8, false));
+      ARROW_ASSIGN_OR_RAISE(std::shared_ptr<arrow::Buffer> offsets, alloc((n + 1) * (large ? 8 : 4) + 8, false));
       ARROW_ASSIGN_OR_RAISE(std::shared_ptr<arrow::Buffer> bytes, alloc(need + 8, false));
       outs[i].values = reinterpret_cast<void*>(offsets->address());
       outs[i].var_data = reinterpret_cast<void*>(bytes->address());

@@ -254,6 +254,16 @@ GDV_DEV gdv_str gdv_sv_view(const uint4& v, const uint4* at, const u8* const* bu
   const u8* base = reinterpret_cast<const u8*>(__ldg(reinterpret_cast<const unsigned long long*>(bufs) + bi));
   return gdv_make_str(base + off, len);
 }
+// Row of a large_string / large_binary column from its int64 offsets [sb, se) into `base` (the data
+// buffer, or the string stage rebased so that base + offset lands on the staged bytes).  A length
+// outside [0, INT32_MAX] does not fit gdv_str.len: the row is invalid input here, reads as null
+// (*ok = false) and as the empty string, and nothing is dereferenced for it.
+GDV_DEV gdv_str gdv_large_str(const u8* base, i64 sb, i64 se, bool* ok) {
+  const i64 len = se - sb;
+  const bool good = len >= 0 && len <= 0x7fffffffll;
+  *ok = good;
+  return gdv_make_str(good ? base + sb : base, good ? (i32)len : 0);
+}
 // Mask of the first k bytes (k clamped to [0, 4]) of a little-endian word.
 GDV_DEV u32 gdv_bytemask(i32 k) { return k <= 0 ? 0u : k >= 4 ? 0xffffffffu : (1u << (8 * k)) - 1u; }
 // Bytes [4, n) of a string against bytes [4, n) of a literal (the first four agreed already).

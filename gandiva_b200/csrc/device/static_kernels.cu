@@ -86,13 +86,15 @@ extern "C" __global__ void __launch_bounds__(256) gdv_fill_u32(u32* p, i64 words
 // ---- string-producing projections: exclusive scan of the per-tile byte counts -------------------
 // One CTA of 1024 threads walks the tile array in blocks of 1024 (a 1e9-row batch has ~2M tiles of
 // 512 rows: a few hundred microseconds next to the two passes over the string bytes).  Writes the
-// total to *total; above `limit` it raises GDV_ERR_OFFSET_OVERFLOW when the total does not fit int32
-// offsets, else GDV_ERR_VAR_CAPACITY (`limit` is then the caller's var_data capacity).
+// total to *total; above `limit` it raises GDV_ERR_OFFSET_OVERFLOW when the total exceeds
+// `offset_limit` (2^31 - 1 for int32 offsets, no limit for the int64 offsets of large_string /
+// large_binary outputs), else GDV_ERR_VAR_CAPACITY (`limit` is then the caller's var_data capacity).
 // With `n_ptr` (a slot count in device memory, gdv_selection_t.d_num_slots) only the tiles that hold
 // its first min(*n_ptr, n_tiles * tile_rows) rows are scanned: the sizing pass wrote no others, and a
 // selective Filter leaves far fewer tiles than the host-side bound this one CTA would otherwise walk.
 extern "C" __global__ void __launch_bounds__(1024)
-gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit, const u64* n_ptr, i64 tile_rows) {
+gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit, const u64* n_ptr, i64 tile_rows,
+               u64 offset_limit) {
   __shared__ u64 s_warp[32];
   __shared__ u64 s_carry;
   const u32 lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
@@ -131,7 +133,7 @@ gdv_scan_tiles(u64* tiles, i64 n_tiles, u64* total, int* err, u64 limit, const u
   if (threadIdx.x == 0) {
     *total = s_carry;
     if (s_carry > limit && err != nullptr)
-      atomicCAS(err, 0, s_carry > 0x7fffffffull ? GDV_ERR_OFFSET_OVERFLOW : GDV_ERR_VAR_CAPACITY);
+      atomicCAS(err, 0, s_carry > offset_limit ? GDV_ERR_OFFSET_OVERFLOW : GDV_ERR_VAR_CAPACITY);
   }
 }
 

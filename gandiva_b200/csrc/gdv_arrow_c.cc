@@ -68,6 +68,16 @@ Status ParseFormat(const char* f, DataType* out) {
   return Status::Make(GDV_NOT_IMPLEMENTED, "Arrow format string '" + s + "' is not supported");
 }
 
+// The Arrow C Device interface speaks int32-offset utf8 / binary only: a projector with a
+// large_string / large_binary result is refused there.
+Status RefuseLargeOutputs(const std::vector<ExpressionPtr>& exprs) {
+  for (const auto& e : exprs)
+    if (e->result().type.is_large())
+      return Status::Make(GDV_NOT_IMPLEMENTED, "output '" + e->result().name + "' is " + e->result().type.ToString() +
+                                                   ": the Arrow C Device interface takes utf8 / binary outputs only");
+  return Status::OK();
+}
+
 std::string FormatOf(const DataType& t) {
   static const char kUnit[] = {'s', 'm', 'u', 'n'};
   if (t.is_view()) return t.id == GDV_TYPE_BINARY ? "vz" : "vu";
@@ -331,6 +341,7 @@ void gdv_arrow_batch_release(gdv_arrow_batch_t batch) {
 gdv_status gdv_projector_output_schema_arrow(gdv_projector_t p, struct ArrowSchema* out) {
   if (p == nullptr || out == nullptr) return Fail(GDV_INVALID, "null argument");
   const auto& exprs = reinterpret_cast<ProjH*>(p)->p->expressions();
+  if (Status s = RefuseLargeOutputs(exprs); !s.ok()) return Fail(s);
   SchemaPriv* priv = new SchemaPriv();
   const size_t n = exprs.size();
   priv->formats.reserve(n);
@@ -363,6 +374,7 @@ gdv_status gdv_projector_evaluate_arrow(gdv_projector_t p, gdv_arrow_batch_t bat
                                         struct ArrowDeviceArray* out) {
   if (p == nullptr || batch == nullptr || out == nullptr) return Fail(GDV_INVALID, "null argument");
   Projector& pr = *reinterpret_cast<ProjH*>(p)->p;
+  if (Status s = RefuseLargeOutputs(pr.expressions()); !s.ok()) return Fail(s);
   const bool device = batch->view.mem_space == GDV_MEM_DEVICE;
   if (device && batch->device != pr.config().device)
     return Fail(GDV_INVALID, "the batch lives on device " + std::to_string(batch->device) +

@@ -31,6 +31,13 @@ Status ViewResult(const std::string& what, const DataType& t) {
                                            " outputs are not supported (results are plain utf8 / binary)");
 }
 
+// large_string / large_binary is a layout of a column or of an expression's result field; a node that
+// computes a value yields plain utf8 / binary (the output's offsets are widened when it is written).
+Status LargeResult(const std::string& what, const DataType& t) {
+  return Status::Make(GDV_NOT_IMPLEMENTED, "'" + what + "' has a " + t.ToString() + " return type: only a field or an "
+                                           "expression's result may be " + t.ToString() + " (nodes yield utf8 / binary)");
+}
+
 bool IsSupportedType(const DataType& t) {
   switch (t.id) {
     case GDV_TYPE_BOOL: case GDV_TYPE_UINT8: case GDV_TYPE_INT8: case GDV_TYPE_UINT16:
@@ -88,12 +95,14 @@ Status ValidateNode(const Schema& schema, const Node& node) {
       if (!IsSupportedType(node.return_type()) || node.return_type().is_dict() || node.return_type().is_view())
         return VErr("Value " + node.ToString() + " has unsupported data type " +
                     node.return_type().ToString());
+      if (node.return_type().is_large()) return LargeResult("literal", node.return_type());
       return Status::OK();
     }
     case NodeKind::kFunction: {
       const auto& fn = static_cast<const FunctionNode&>(node);
       if (fn.return_type().is_dict()) return DictionaryResult(fn.name());
       if (fn.return_type().is_view()) return ViewResult(fn.name(), fn.return_type());
+      if (fn.return_type().is_large()) return LargeResult(fn.name(), fn.return_type());
       std::vector<DataType> params;
       for (const auto& c : fn.children()) {
         Status s = ValidateNode(schema, *c);
@@ -175,6 +184,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
       const auto& n = static_cast<const IfNode&>(node);
       if (n.return_type().is_dict()) return DictionaryResult("if");
       if (n.return_type().is_view()) return ViewResult("if", n.return_type());
+      if (n.return_type().is_large()) return LargeResult("if", n.return_type());
       for (const NodePtr* c : {&n.condition(), &n.then_node(), &n.else_node()}) {
         Status s = ValidateNode(schema, **c);
         if (!s.ok()) return s;
@@ -1547,7 +1557,8 @@ void EmitPrologue(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, 
       *o += "  const i64* in_vsz" + J + " = A.in_vsz[" + J + "];\n";
       *o += "  const i64 in_vbn" + J + " = A.in_vbn[" + J + "];\n";
     } else if (t.is_varlen()) {
-      *o += "  const i32* in_val" + J + " = reinterpret_cast<const i32*>(A.in_val[" + J + "]);\n";
+      const std::string ot = t.is_large() ? "i64" : "i32";
+      *o += "  const " + ot + "* in_val" + J + " = reinterpret_cast<const " + ot + "*>(A.in_val[" + J + "]);\n";
       *o += "  const u8* in_var" + J + " = A.in_var[" + J + "];\n";
     } else {
       *o += "  const " + std::string(t.ctype()) + "* in_val" + J + " = reinterpret_cast<const " +
@@ -1688,6 +1699,7 @@ std::string EmitCoopScan(int j, const std::vector<CoopSeg>& segs, int R, const s
     o += I + "        i32 rs = 0, re = -1;\n";
     o += I + "        #pragma unroll\n";
     o += I + "        for (int k = 0; k < " + std::to_string(R) + "; ++k) {\n";
+    // (large column: ptr and gb are i64; the group's bytes fit the stage, so the difference fits i32)
     o += I + "          const i32 a = ptr" + J + "[32 * k] - gb + (i32)mis;\n";
     o += I + "          const i32 b = ptr" + J + "[32 * k + 1] - gb + (i32)mis;\n";
     o += I + "          const u32 own = __ballot_sync(GDV_FULL, a <= p && p + " + KL + " <= b);\n";
@@ -1767,7 +1779,9 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
       *o += I + "uint4 w" + std::to_string(j) + "[" + sR + "];\n";
       *o += I + "bool d" + std::to_string(j) + "[" + sR + "];\n";
     } else if (t.is_varlen()) {
-      // group state of the string stage: rows known to be ASCII, cooperative-scan hit list usable
+      // group state of the string stage: rows known to be ASCII, cooperative-scan hit list usable;
+      // large column: whether each row's length fits a gdv_str (gdv_large_str)
+      if (t.is_large()) *o += I + "bool d" + std::to_string(j) + "[" + sR + "];\n";
       *o += I + "u32 ascii" + std::to_string(j) + " = 0u;\n";
       if (SlotHasCoop(coop, static_cast<int>(j))) {
         *o += I + "bool coop" + std::to_string(j) + " = false;\n";
@@ -1798,6 +1812,7 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
         *o += I + "const " +
               (t.is_dict()   ? std::string(DataType(t.index).ctype())
                : t.is_view() ? std::string("uint4")
+               : t.is_large() ? std::string("i64")
                : t.is_varlen() ? std::string("i32") : std::string(t.ctype())) +
               "* ptr" + J + " = in_val" + J + " + base + (i64)lane;\n";
       if (HasByteRun(slots[j]) && stage_bytes > 0) {
@@ -1807,11 +1822,21 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
         staged_any = true;
         *o += I + "const u8* sbase" + J + " = in_var" + J + ";\n";
         *o += I + "{\n";
-        *o += I + "  const i32 gb = in_val" + J + "[base];\n";
-        *o += I + "  const i32 gn = in_val" + J + "[base + " + std::to_string(32 * R) + "] - gb;\n";
-        *o += I + "  const u8* src = in_var" + J + " + gb;\n";
-        *o += I + "  const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
-        *o += I + "  if (gn + (i32)mis <= " + std::to_string(stage_bytes) + ") {\n";
+        if (t.is_large()) {
+          // int64 offsets: the run is measured in i64 and narrowed once it is known to fit the stage
+          *o += I + "  const i64 gb = in_val" + J + "[base];\n";
+          *o += I + "  const i64 gn64 = in_val" + J + "[base + " + std::to_string(32 * R) + "] - gb;\n";
+          *o += I + "  const u8* src = in_var" + J + " + gb;\n";
+          *o += I + "  const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
+          *o += I + "  if (gn64 + (i64)mis <= " + std::to_string(stage_bytes) + ") {\n";
+          *o += I + "    const i32 gn = (i32)gn64;\n";
+        } else {
+          *o += I + "  const i32 gb = in_val" + J + "[base];\n";
+          *o += I + "  const i32 gn = in_val" + J + "[base + " + std::to_string(32 * R) + "] - gb;\n";
+          *o += I + "  const u8* src = in_var" + J + " + gb;\n";
+          *o += I + "  const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
+          *o += I + "  if (gn + (i32)mis <= " + std::to_string(stage_bytes) + ") {\n";
+        }
         *o += I + "    const i32 nchunks = (gn + (i32)mis + 15) >> 4;\n";
         *o += I + "    u32 hibits = 0u;\n";
         if (!prefetched) {
@@ -1863,6 +1888,9 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
       } else if (t.is_view()) {
         *o += I + "  w" + J + "[k] = gdv_ldview(ptr" + J + " + 32 * k);\n";
         *o += I + "  f" + J + "[k] = " + SvView(J, "ptr" + J + " + 32 * k") + ";\n";
+      } else if (t.is_large()) {
+        *o += I + "  { f" + J + "[k] = gdv_large_str(" + (stage_bytes > 0 ? "sbase" : "in_var") + J + ", ptr" + J +
+              "[32 * k], ptr" + J + "[32 * k + 1], &d" + J + "[k]); f" + J + "[k].xf = ascii" + J + "; }\n";
       } else if (t.is_varlen()) {
         *o += I + "  { const i32 sb = ptr" + J + "[32 * k]; const i32 se = ptr" + J +
               "[32 * k + 1]; f" + J + "[k] = gdv_make_str(" +
@@ -1883,7 +1911,8 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
         else
           *o += I + "  k" + J + "[k] = ((gdv_ldwin(in_vp" + J + ", ((base >> 5) + k) & in_vm" + J + ", in_vsh" +
                 J + ") >> lane) & 1u) != 0u" +
-                (slots[j].type.is_dict() || slots[j].type.is_view() ? " && d" + J + "[k]" : "") + ";\n";
+                (slots[j].type.is_dict() || slots[j].type.is_view() || slots[j].type.is_large() ? " && d" + J + "[k]" : "") +
+                ";\n";
       }
       *o += I + "}\n";
     }
@@ -1904,6 +1933,9 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
       } else if (t.is_view()) {
         *o += I + "  w" + J + "[k] = in ? gdv_ldview(in_val" + J + " + r) : make_uint4(0u, 0u, 0u, 0u);\n";
         *o += I + "  f" + J + "[k] = " + SvView(J, "in_val" + J + " + r") + ";\n";
+      } else if (t.is_large()) {
+        *o += I + "  f" + J + "[k] = gdv_large_str(in_var" + J + ", in ? in_val" + J + "[r] : 0ll, in ? in_val" + J +
+              "[r + 1] : 0ll, &d" + J + "[k]);\n";
       } else if (t.is_varlen()) {
         *o += I + "  { const i32 sb = in ? in_val" + J + "[r] : 0; const i32 se = in ? in_val" + J +
               "[r + 1] : 0; f" + J + "[k] = gdv_make_str(in_var" + J + " + sb, se - sb); }\n";
@@ -1914,7 +1946,8 @@ void EmitGroup(const std::vector<ColumnSlot>& slots, const KernelSpec& spec, boo
         *o += I + "  k" + J + "[k] = in;\n";
       else if (spec.nullable)
         *o += I + "  k" + J + "[k] = in && (!in_hv" + J + " || gdv_ldbit(reinterpret_cast<const u8*>(in_vld" +
-              J + "), in_vsh" + J + ", r))" + (t.is_dict() || t.is_view() ? " && d" + J + "[k]" : "") + ";\n";
+              J + "), in_vsh" + J + ", r))" + (t.is_dict() || t.is_view() || t.is_large() ? " && d" + J + "[k]" : "") +
+              ";\n";
     }
     *o += I + "}\n";
   }
@@ -2248,7 +2281,7 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
   __shared__ u32 s_wcount[@NW@];
   __shared__ i64 s_tile;
   __shared__ u64 s_excl;
-  const i32* const offs = in_val@J@;
+  const @OFFT@* const offs = in_val@J@;
   const u8* const data = in_var@J@;
   const i64 n_tiles = (A.n + @TILE@ - 1) / @TILE@;
   const i64 B0 = (i64)offs[0], B1 = (i64)offs[A.n];
@@ -2276,7 +2309,7 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
       const i64 b0 = (i64)offs[r0], b1 = (i64)offs[r1];
       auto push = [&](i64 pos) {
         const u32 ix = atomicAdd(wctr, 1u);
-        if (ix < @CAP@u) wanch[ix] = (u32)pos;
+        if (ix < @CAP@u) wanch[ix] = (u32)@ANCHOR@;
       };
       // bytes of this run that share a chunk with memory outside the column: every one is an anchor
       i64 c_lo = (b0 + mis) >> 4, c_hi = (b1 + mis + 15) >> 4;
@@ -2298,10 +2331,10 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
       // of it a match), the warp goes over its rows a second time, 128 rows per step, with the first
       // byte of every non-empty row as its anchor.
       const uint4* const cp = abase + c_lo + (i64)lane;
-      const i32 nch = c_hi > c_lo ? (i32)(c_hi - c_lo) : 0;
+      const i32 nch = @NCH@;
       i32 ci = 0;
       i64 redo_row = r0;
-      bool redo = false, lost = false;
+      bool redo = false, lost = @LOST@;
       while (true) {
         bool last;
         if (!redo) {
@@ -2345,9 +2378,7 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
           for (int u = 0; u < 4; ++u) {
             const i64 row = redo_row + 32 * u + (i64)lane;
             if (row < r1) {
-              const i32 a = __ldg(offs + row);
-              if (__ldg(offs + row + 1) > a) push((i64)a);
-            }
+@REDO_PUSH@            }
           }
           redo_row += 128;
           last = redo_row >= r1;
@@ -2361,17 +2392,7 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
           const u32 nc = queued < @CAP@u ? queued : @CAP@u;
           for (u32 i0 = 0u; i0 < nc; i0 += 32u) {
             const bool has = i0 + lane < nc;
-            const i64 pos = has ? (i64)wanch[i0 + lane] : b0;
-            // last row r in [r0, r1) with offs[r] <= pos (offsets are non-decreasing; empty rows are skipped)
-            i64 lo = r0, hi = r1;
-            while (hi - lo > 1) {
-              const i64 mid = (lo + hi) >> 1;
-              if ((i64)__ldg(offs + mid) <= pos) lo = mid;
-              else hi = mid;
-            }
-            const u32 rr = (u32)(lo - r0);
-            const bool cand = has && pos >= b0 && pos < b1 && ((wmask[rr >> 5] >> (rr & 31u)) & 1u) == 0u;
-            bool keep = false;
+@DRAIN_ROW@            bool keep = false;
             {
               const i64 base = (cand ? lo : A.n) - (i64)lane;
 @PRED@            }
@@ -2438,6 +2459,52 @@ std::string EmitKeyFilter(const std::vector<ColumnSlot>& slots, const KernelSpec
   ReplaceAll(&k, "@W@", std::to_string(W));
   ReplaceAll(&k, "@IDX@", SelCType(spec.selection_mode));
   ReplaceAll(&k, "@UNIT@", std::to_string(unit));
+  // Anchor positions are u32.  A utf8 / binary column's are absolute; a large column's are relative to
+  // the warp's run base b0, and in the fallback (redo) the list holds rows relative to r0 instead of
+  // first bytes, so no position past the u32 range is ever stored.  A run longer than a u32 position
+  // can address skips the streaming loop and goes to the fallback: every row of the run is evaluated.
+  const bool large = slots[static_cast<size_t>(plan.slot)].type.is_large();
+  ReplaceAll(&k, "@OFFT@", large ? "i64" : "i32");
+  ReplaceAll(&k, "@ANCHOR@", large ? "(pos - b0)" : "pos");
+  ReplaceAll(&k, "@NCH@", large ? "c_hi > c_lo && b1 - b0 <= 0xffffffffll ? (i32)(c_hi - c_lo) : 0"
+                                : "c_hi > c_lo ? (i32)(c_hi - c_lo) : 0");
+  ReplaceAll(&k, "@LOST@", large ? "b1 - b0 > 0xffffffffll" : "false");
+  if (large) {
+    ReplaceAll(&k, "@REDO_PUSH@",
+               "              if (__ldg(offs + row + 1) > __ldg(offs + row)) push(b0 + (row - r0));  // stores row - r0\n");
+    ReplaceAll(&k, "@DRAIN_ROW@",
+               "            const i64 pos = has ? b0 + (i64)wanch[i0 + lane] : b0;\n"
+               "            // fallback: the list holds rows; else the last row r in [r0, r1) with offs[r] <= pos\n"
+               "            // (offsets are non-decreasing; empty rows are skipped)\n"
+               "            i64 lo = r0, hi = r1;\n"
+               "            if (redo) {\n"
+               "              lo = r0 + (pos - b0);\n"
+               "            } else {\n"
+               "              while (hi - lo > 1) {\n"
+               "                const i64 mid = (lo + hi) >> 1;\n"
+               "                if (__ldg(offs + mid) <= pos) lo = mid;\n"
+               "                else hi = mid;\n"
+               "              }\n"
+               "            }\n"
+               "            const u32 rr = (u32)(lo - r0);\n"
+               "            const bool cand = has && (redo ? lo < r1 : pos >= b0 && pos < b1) &&\n"
+               "                              ((wmask[rr >> 5] >> (rr & 31u)) & 1u) == 0u;\n");
+  } else {
+    ReplaceAll(&k, "@REDO_PUSH@", R"K(              const i32 a = __ldg(offs + row);
+              if (__ldg(offs + row + 1) > a) push((i64)a);
+)K");
+    ReplaceAll(&k, "@DRAIN_ROW@", R"K(            const i64 pos = has ? (i64)wanch[i0 + lane] : b0;
+            // last row r in [r0, r1) with offs[r] <= pos (offsets are non-decreasing; empty rows are skipped)
+            i64 lo = r0, hi = r1;
+            while (hi - lo > 1) {
+              const i64 mid = (lo + hi) >> 1;
+              if ((i64)__ldg(offs + mid) <= pos) lo = mid;
+              else hi = mid;
+            }
+            const u32 rr = (u32)(lo - r0);
+            const bool cand = has && pos >= b0 && pos < b1 && ((wmask[rr >> 5] >> (rr & 31u)) & 1u) == 0u;
+)K");
+  }
   return k;
 }
 
@@ -2471,8 +2538,8 @@ void ApplyDeviceCount(std::string* src) {
 void MarkHoisted(const BodyGen& gen, const Node& cond, std::vector<ColumnSlot>* slots) {
   std::vector<int> strict;
   gen.TruthStrict(cond, &strict);
-  for (auto& sl : *slots)  // a dictionary / view row's validity also depends on its entry / view: read per row
-    if (!sl.type.is_dict() && !sl.type.is_view() && std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end())
+  for (auto& sl : *slots)  // a dictionary / view / large row's validity also depends on its entry / view / length
+    if (!sl.type.is_dict() && !sl.type.is_view() && !sl.type.is_large() && std::find(strict.begin(), strict.end(), sl.schema_index) != strict.end())
       sl.hoist = true;
 }
 
@@ -2565,6 +2632,7 @@ int InBytesPerRow(const std::vector<ColumnSlot>& slots) {
   for (const auto& s : slots)
     bytes += s.type.is_dict() ? DataType(s.type.index).width()  // the index; the dictionary is cached
              : s.type.is_view()   ? 16                               // the view; out-of-line bytes on demand
+             : s.type.is_large()  ? 36                               // 8 B offset + ~28 B data
              : s.type.is_varlen() ? 32 : std::max(s.type.width(), 1);  // 4 B offset + ~28 B data
   return bytes;
 }
@@ -2698,6 +2766,10 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   out->rows_per_thread = R;
   out->block_threads = BT;
   const std::string sR = std::to_string(R), s32R = std::to_string(32 * R), sT = std::to_string(T);
+  // large_string / large_binary output: int64 offsets, and the running byte counts inside a thread and
+  // a warp are u64 (the totals across warps and tiles already are)
+  const bool large_out = expr->result().type.is_large();
+  const std::string OFF = large_out ? "i64" : "i32", RUN = large_out ? "u64" : "u32";
 
   std::string header = HeaderLines(is_size ? "string projection, sizing pass" : "string projection, write pass", spec, {expr});
   if (gen.has_replace()) header += "#define GDV_HAS_REPL 1\n";
@@ -2705,7 +2777,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   if (st.stage_bytes > 0) src += EmitStageDecls(slots, gen.coop_segs(), st, "u8* ", "", ";\n");
   src += "  __shared__ u64 s_part[" + std::to_string(NW) + "];\n";
   if (has_sel && !is_size)  // a device count of 0 leaves no tile to write offsets[0]
-    src += "  if (A.n == 0 && blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<i32*>(A.out_val[0])[0] = 0;\n";
+    src += "  if (A.n == 0 && blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<" + OFF + "*>(A.out_val[0])[0] = 0;\n";
   src += "  const i64 n_tiles = (A.n + " + std::to_string(T - 1) + ") / " + sT + ";\n";
   src += "  for (i64 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {\n";
   src += "    const i64 base = tile * " + sT + " + (i64)wid * " + s32R + ";\n";
@@ -2718,8 +2790,8 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   for (int i = 0; i < K; ++i) total_len += (i ? " + " : "") + std::string("gdv_piece_len(") + parts[i] + ")";
   std::string tail;
   if (is_size) {
-    src += "    u32 tsum = 0u;\n";
-    tail = "        tsum += (in && (" + res.ok + ")) ? (" + total_len + ") : 0u;\n";
+    src += "    " + RUN + " tsum = 0u;\n";
+    tail = "        tsum += (in && (" + res.ok + ")) ? " + (large_out ? "(u64)(" : "(") + total_len + ") : 0u;\n";
   } else {
     src += "    u32 slen[" + sR + "];\n    gdv_str sv[" + sR + "][" + sK + "];\n    u32 vw0 = 0u;\n";
     tail = "        { const bool okk = in && (" + res.ok + "); slen[k] = okk ? (" + total_len + ") : 0u;\n";
@@ -2751,14 +2823,14 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
     src += "    __syncthreads();\n";
   } else {
     // lengths -> inclusive offsets inside the warp (row order: step k, then lane), then across warps
-    src += "    u32 incl[" + sR + "];\n";
-    src += "    u32 run = 0u;\n";
+    src += "    " + RUN + " incl[" + sR + "];\n";
+    src += "    " + RUN + " run = 0u;\n";
     src += "    #pragma unroll\n";
     src += "    for (int k = 0; k < " + sR + "; ++k) {\n";
-    src += "      u32 x = slen[k];\n";
+    src += "      " + RUN + " x = slen[k];\n";
     src += "      #pragma unroll\n";
     src += "      for (int o = 1; o < 32; o <<= 1) {\n";
-    src += "        const u32 t = __shfl_up_sync(GDV_FULL, x, o);\n";
+    src += "        const " + RUN + " t = __shfl_up_sync(GDV_FULL, x, o);\n";
     src += "        if (lane >= (u32)o) x += t;\n";
     src += "      }\n";
     src += "      incl[k] = run + x;\n";
@@ -2769,12 +2841,12 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
     src += "    u64 wbase = A.tile_state[tile];\n";
     src += "    for (u32 w = 0u; w < wid; ++w) wbase += s_part[w];\n";
     src += "    __syncthreads();\n";
-    src += "    i32* offs = reinterpret_cast<i32*>(A.out_val[0]);\n";
+    src += "    " + OFF + "* offs = reinterpret_cast<" + OFF + "*>(A.out_val[0]);\n";
     src += "    u8* data = A.out_var[0];\n";
     src += "    #pragma unroll\n";
     src += "    for (int k = 0; k < " + sR + "; ++k) {\n";
     src += "      const i64 s = base + 32 * k + (i64)lane;\n";
-    src += "      if (s < A.n) offs[s + 1] = (i32)(wbase + (u64)incl[k]);\n";
+    src += "      if (s < A.n) offs[s + 1] = (" + OFF + ")(wbase + (u64)incl[k]);\n";
     src += "    }\n";
     src += "    if (tile == 0 && threadIdx.x == 0) offs[0] = 0;\n";
     src += "    #pragma unroll\n";
@@ -2825,7 +2897,7 @@ Status GenerateStringKernel(const Schema& schema, const ExpressionPtr& expr, con
   out->source = std::move(src);
   out->outputs = {expr->result().type};
   out->uses_ctx = gen.uses_ctx() || !is_size;
-  out->out_bytes_per_row = 4;
+  out->out_bytes_per_row = large_out ? 8 : 4;
   out->dynamic_smem = st.dynamic_smem(BT);
   out->tile_rows = T;
   out->cta_tile_rows = T;
@@ -2923,11 +2995,20 @@ void EmitPrefetchLoop(const std::vector<ColumnSlot>& slots, const KernelSpec& sp
     if (!HasByteRun(slots[j])) continue;
     const std::string J = std::to_string(j);
     src += "      {\n";
-    src += "        const i32 gb = in_val" + J + "[b];\n";
-    src += "        const i32 gn = in_val" + J + "[b + " + s32R + "] - gb;\n";
-    src += "        const u8* src = in_var" + J + " + gb;\n";
-    src += "        const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
-    src += "        if (gn + (i32)mis <= " + std::to_string(stage_bytes) + ") {\n";
+    if (slots[j].type.is_large()) {  // as in EmitGroup: i64 run, narrowed once it fits the stage
+      src += "        const i64 gb = in_val" + J + "[b];\n";
+      src += "        const i64 gn64 = in_val" + J + "[b + " + s32R + "] - gb;\n";
+      src += "        const u8* src = in_var" + J + " + gb;\n";
+      src += "        const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
+      src += "        if (gn64 + (i64)mis <= " + std::to_string(stage_bytes) + ") {\n";
+      src += "          const i32 gn = (i32)gn64;\n";
+    } else {
+      src += "        const i32 gb = in_val" + J + "[b];\n";
+      src += "        const i32 gn = in_val" + J + "[b + " + s32R + "] - gb;\n";
+      src += "        const u8* src = in_var" + J + " + gb;\n";
+      src += "        const u32 mis = (u32)((unsigned long long)src & 15ull);\n";
+      src += "        if (gn + (i32)mis <= " + std::to_string(stage_bytes) + ") {\n";
+    }
     src += "          const i32 nchunks = (gn + (i32)mis + 15) >> 4;\n";
     src += "          u8* dst = stage" + J + "_0 + (size_t)par * " + std::to_string(stage_bytes) + "u;\n";
     src += "          for (i32 c = (i32)lane; c < nchunks; c += 32)\n";
@@ -3396,10 +3477,11 @@ NodePtr WithValueTypes(const NodePtr& node) {
   return WithChildren(node, std::move(kids));
 }
 
-static bool ReadsDictionaryOrView(const Node& node) {
-  if (node.kind() == NodeKind::kField) return node.return_type().is_dict() || node.return_type().is_view();
+static bool ReadsRowCheckedColumn(const Node& node) {
+  if (node.kind() == NodeKind::kField)
+    return node.return_type().is_dict() || node.return_type().is_view() || node.return_type().is_large();
   for (const auto& c : Children(node))
-    if (ReadsDictionaryOrView(*c)) return true;
+    if (ReadsRowCheckedColumn(*c)) return true;
   return false;
 }
 
@@ -3410,9 +3492,10 @@ Status GenerateKernel(const Schema& schema, const std::vector<ExpressionPtr>& ex
   for (const auto& e : exprs) {
     NodePtr r = RewriteAliases(e->root());
     lowered.push_back(r == e->root() ? e : std::make_shared<Expression>(r, e->result()));
-    // a dictionary row is null when its entry is, or when its index is out of range, and a view row
-    // when its view is invalid: such kernels always keep the validity plumbing
-    if (ReadsDictionaryOrView(*r)) s.nullable = true;
+    // a dictionary row is null when its entry is, or when its index is out of range, a view row
+    // when its view is invalid, and a large row when its length does not fit a gdv_str: such kernels
+    // always keep the validity plumbing
+    if (ReadsRowCheckedColumn(*r)) s.nullable = true;
   }
   if (s.kind == KernelKind::kStringSize || s.kind == KernelKind::kStringWrite) {
     if (lowered.size() != 1 || !lowered[0]->result().type.is_varlen())

@@ -6,6 +6,7 @@
 namespace gdv {
 
 int DataType::width() const {
+  if (large) return 8;
   switch (id) {
     case GDV_TYPE_BOOL: return 0;
     case GDV_TYPE_UINT8: case GDV_TYPE_INT8: return 1;
@@ -31,6 +32,7 @@ static const char* unit_name(int u) {
 
 std::string DataType::ToString() const {
   if (view) return id == GDV_TYPE_BINARY ? "binary_view" : "string_view";
+  if (large) return id == GDV_TYPE_BINARY ? "large_binary" : "large_string";
   if (index != 0)
     return "dictionary<values=" + value_type().ToString() + ", indices=" + DataType(index).ToString() +
            ", ordered=" + (ordered ? "1" : "0") + ">";

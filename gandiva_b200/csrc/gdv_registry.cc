@@ -75,7 +75,7 @@ namespace {
 thread_local const FunctionRegistry* tl_user_functions = nullptr;
 
 bool IsUserValueType(const DataType& t, bool allow_varlen) {
-  if (t.is_dict() || t.is_view()) return false;
+  if (t.is_dict() || t.is_view() || t.is_large()) return false;
   switch (t.id) {
     case GDV_TYPE_BOOL: case GDV_TYPE_UINT8: case GDV_TYPE_INT8: case GDV_TYPE_UINT16: case GDV_TYPE_INT16:
     case GDV_TYPE_UINT32: case GDV_TYPE_INT32: case GDV_TYPE_UINT64: case GDV_TYPE_INT64: case GDV_TYPE_FLOAT:

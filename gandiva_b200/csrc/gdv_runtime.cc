@@ -613,11 +613,16 @@ Status ResolveInputs(Device* dev, const GeneratedKernel& gen, const gdv_batch_t*
                                      "device views buffer of column %d is not 16-byte aligned", col, &r.val));
       GDV_RETURN_NOT_OK(ResolveViewBuffers(dev, col, c, host, stream, scratch, &r));
     } else if (t.is_varlen()) {
-      const int32_t* offs = static_cast<const int32_t*>(c.values) + off;
-      GDV_RETURN_NOT_OK(ResolveArray(dev, offs, static_cast<size_t>(n + 1) * 4, 0, 1, host, stream, scratch, nullptr, col,
+      // n + 1 offsets of t.width() bytes (int32, or int64 for a large column)
+      const int w = t.width();
+      const uint8_t* offs = values + off * w;
+      auto at = [&](int64_t i) -> int64_t {
+        return t.is_large() ? reinterpret_cast<const int64_t*>(offs)[i] : reinterpret_cast<const int32_t*>(offs)[i];
+      };
+      GDV_RETURN_NOT_OK(ResolveArray(dev, offs, static_cast<size_t>(n + 1) * w, 0, 1, host, stream, scratch, nullptr, col,
                                      &r.val));
       if (host) {
-        const int64_t first = n > 0 ? offs[0] : 0, last = n > 0 ? offs[n] : 0;
+        const int64_t first = n > 0 ? at(0) : 0, last = n > 0 ? at(n) : 0;
         GDV_RETURN_NOT_OK(ResolveArray(dev, static_cast<const uint8_t*>(c.var_data) + first,
                                        static_cast<size_t>(last - first), 16, 1, host, stream, scratch, nullptr, col,
                                        &r.var));
@@ -991,11 +996,12 @@ Status Projector::KernelFor(bool nullable, CompiledKernel** out) {
   return Status::OK();
 }
 
-// True when some column the kernel reads carries a validity bitmap, or is dictionary-encoded or a
-// view column (a row is also null where its dictionary entry is, or where its view is invalid).
+// True when some column the kernel reads carries a validity bitmap, or is dictionary-encoded, a view
+// column or a large column (a row is also null where its dictionary entry is, where its view is
+// invalid, or where its length does not fit a gdv_str).
 static bool AnyValidity(const GeneratedKernel& gen, const gdv_batch_t* batch) {
   for (const auto& slot : gen.inputs)
-    if (slot.type.is_dict() || slot.type.is_view() || (slot.schema_index >= 0 && slot.schema_index < batch->num_columns &&
+    if (slot.type.is_dict() || slot.type.is_view() || slot.type.is_large() || (slot.schema_index >= 0 && slot.schema_index < batch->num_columns &&
                                 batch->columns[slot.schema_index].validity != nullptr))
       return true;
   return false;
@@ -1123,6 +1129,9 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   const DriverApi& d = Driver();
   CUstream stream = stream_v != nullptr ? static_cast<CUstream>(stream_v) : dev->stream();
   const GeneratedKernel& gen = ksize->gen;  // both kernels read the same input slots
+  // a large_string / large_binary output has int64 offsets and no 2^31 - 1 byte limit (code 2)
+  const bool large_out = kwrite->gen.outputs.at(0).is_large();
+  const size_t off_w = large_out ? 8 : 4;
 
   ScratchScope scratch(dev);
   scratch.Guard(stream);
@@ -1160,9 +1169,10 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
     CUdeviceptr tiles = d_state + 16, total = d_state, errp = d_err;
     CUdeviceptr n_ptr = dev_count ? reinterpret_cast<CUdeviceptr>(sel->d_num_slots) : 0;
     int64_t nt = n_tiles, tile_rows = T;
-    uint64_t limit = 0x7fffffffull;
+    uint64_t offset_limit = large_out ? ~0ull : 0x7fffffffull;  // the largest total the output's offsets hold
+    uint64_t limit = offset_limit;
     if (dev_count && !size_only) limit = std::min<uint64_t>(limit, static_cast<uint64_t>(out->var_capacity));
-    void* params[] = {&tiles, &nt, &total, &errp, &limit, &n_ptr, &tile_rows};
+    void* params[] = {&tiles, &nt, &total, &errp, &limit, &n_ptr, &tile_rows, &offset_limit};
     g_launch_count.fetch_add(1);
     GDV_RETURN_NOT_OK(CuCheck(d.LaunchKernel(scan, 1, 1, 1, 1024, 1, 1, 0, stream, params, nullptr),
                               "cuLaunchKernel(gdv_scan_tiles)"));
@@ -1171,7 +1181,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   if (size_only || host || !async) {
     GDV_RETURN_NOT_OK(CuCheck(d.MemcpyDtoHAsync(&total, d_state, 8, stream), "D2H total"));
     GDV_RETURN_NOT_OK(CuCheck(d.StreamSynchronize(stream), "cuStreamSynchronize"));
-    if (total > 0x7fffffffull) {
+    if (!large_out && total > 0x7fffffffull) {
       Sync(stream);  // releases the pending blocks; reports the overflow below
       return Status::Make(GDV_EXECUTION_ERROR, ExecutionErrorMessage(2));
     }
@@ -1194,7 +1204,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
                                            " is smaller than the " + std::to_string(total) +
                                            " bytes the output needs (see var_size)");
     }
-    GDV_RETURN_NOT_OK(scratch.Alloc(static_cast<size_t>(n + 1) * 4 + 16, &d_offs));
+    GDV_RETURN_NOT_OK(scratch.Alloc(static_cast<size_t>(n + 1) * off_w + 16, &d_offs));
     GDV_RETURN_NOT_OK(scratch.Alloc(static_cast<size_t>(total) + 16, &d_data));
     if (out->validity != nullptr) GDV_RETURN_NOT_OK(scratch.Alloc(words * 4 + 8, &d_vld));
     out_cap = static_cast<int64_t>(total);
@@ -1210,7 +1220,7 @@ Status Projector::EvaluateString(StringKernels* sk, const gdv_batch_t* batch,
   GDV_RETURN_NOT_OK(LaunchKernel(dev, lwrite, kwrite->gen, args, GridFor(dev, cfg_, lwrite.blocks_per_sm, blocks_needed),
                                  stream));
   if (host) {
-    GDV_RETURN_NOT_OK(StagedDtoH(dev, out->values, d_offs, static_cast<size_t>(n + 1) * 4, stream));
+    GDV_RETURN_NOT_OK(StagedDtoH(dev, out->values, d_offs, static_cast<size_t>(n + 1) * off_w, stream));
     if (total > 0) GDV_RETURN_NOT_OK(StagedDtoH(dev, out->var_data, d_data, static_cast<size_t>(total), stream));
     if (out->validity != nullptr)
       GDV_RETURN_NOT_OK(StagedDtoH(dev, out->validity, d_vld, static_cast<size_t>((n + 7) / 8), stream));

@@ -17,6 +17,9 @@ namespace gdv {
 // `id` is GDV_TYPE_STRING / BINARY and `view` is set, so everything that reads values sees utf8 /
 // binary and only same() and the kernels' row loaders see the 16-byte views.  is_varlen() holds
 // for all three layouts; HasByteRun (gdv_codegen.cc) is what "contiguous offsets + bytes" means.
+// A large_string / large_binary column (arrow::LargeStringType / LargeBinaryType) is utf8 / binary
+// with `large` set: the same contiguous bytes behind int64 offsets.  Unlike the two encodings above
+// it may also be an expression's result type (an output with int64 offsets).
 struct DataType {
   int32_t id = GDV_TYPE_NA;
   int32_t precision = 0;  // decimal precision, or time unit for timestamp/time
@@ -24,6 +27,7 @@ struct DataType {
   int32_t index = 0;      // dictionary columns: GDV_TYPE_INT8..INT64 (or what the caller sent)
   bool ordered = false;   // dictionary columns: DictionaryType::ordered
   bool view = false;      // string_view / binary_view columns
+  bool large = false;     // large_string / large_binary columns and results (int64 offsets)
 
   DataType() = default;
   DataType(int32_t i, int32_t p = 0, int32_t s = 0) : id(i), precision(p), scale(s) {}
@@ -37,19 +41,26 @@ struct DataType {
       id = t.id == GDV_TYPE_STRING_VIEW ? GDV_TYPE_STRING : GDV_TYPE_BINARY;
       view = true;
       precision = scale = 0;
+    } else if (t.id == GDV_TYPE_LARGE_STRING || t.id == GDV_TYPE_LARGE_BINARY) {
+      id = t.id == GDV_TYPE_LARGE_STRING ? GDV_TYPE_STRING : GDV_TYPE_BINARY;
+      large = true;
+      precision = scale = 0;
     }
   }
   gdv_type_t c() const {
     if (view) return gdv_type_t{id == GDV_TYPE_BINARY ? GDV_TYPE_BINARY_VIEW : GDV_TYPE_STRING_VIEW, 0, 0};
+    if (large) return gdv_type_t{id == GDV_TYPE_BINARY ? GDV_TYPE_LARGE_BINARY : GDV_TYPE_LARGE_STRING, 0, 0};
     if (index != 0) return gdv_type_t{GDV_TYPE_DICTIONARY, index | (ordered ? GDV_DICT_ORDERED : 0), id};
     return gdv_type_t{id, precision, scale};
   }
   bool is_dict() const { return index != 0; }
   bool is_view() const { return view; }
-  // The type of the values (the dictionary's type for a dictionary column, utf8 / binary for a view).
+  bool is_large() const { return large; }
+  // The type of the values (the dictionary's type for a dictionary column, utf8 / binary for a view
+  // or a large column).
   DataType value_type() const { return DataType(id, precision, scale); }
   bool same(const DataType& o) const {
-    return *this == o && index == o.index && ordered == o.ordered && view == o.view;
+    return *this == o && index == o.index && ordered == o.ordered && view == o.view && large == o.large;
   }
 
   bool operator==(const DataType& o) const {
@@ -72,7 +83,7 @@ struct DataType {
   }
 
   // Width in bytes of one value in the Arrow values buffer (0 for bool = bit-packed,
-  // 4 for the offsets buffer of utf8/binary).
+  // 4 for the offsets buffer of utf8/binary, 8 for large_string / large_binary).
   int width() const;
   // arrow::DataType::ToString() spelling ("int32", "double", "decimal128(12, 2)", ...).
   std::string ToString() const;

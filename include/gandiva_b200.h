@@ -96,6 +96,13 @@ typedef int32_t gdv_status;
  * type is refused at Make() with GDV_NOT_IMPLEMENTED. */
 #define GDV_TYPE_STRING_VIEW 39
 #define GDV_TYPE_BINARY_VIEW 40
+/* Arrow's int64-offset layouts of utf8 / binary (arrow::LargeStringType, LargeBinaryType; C format
+ * "U" / "Z"): the utf8 / binary layout with int64 offsets, so a column may hold more than 2^31 - 1
+ * bytes.  Functions, IN and if/else resolve against utf8 / binary.  An expression's result field may
+ * be large_string / large_binary when its root yields utf8 / binary; a function, if/else or literal
+ * node with a large return type is refused at Make() with GDV_NOT_IMPLEMENTED. */
+#define GDV_TYPE_LARGE_STRING 34
+#define GDV_TYPE_LARGE_BINARY 35
 
 typedef struct gdv_type {
   int32_t id;        /* GDV_TYPE_* */
@@ -164,6 +171,11 @@ void gdv_config_default(gdv_config_t* cfg);
  *  fixed width : validity | values                (values = buffers[1])
  *  bool        : validity | bit-packed values
  *  utf8/binary : validity | int32 offsets | bytes (values = offsets, var_data = bytes)
+ *  large_string / large_binary : validity | int64 offsets | bytes (values = offsets, var_data = bytes,
+ *                var_data_size).  A non-null row whose length offsets[r+1] - offsets[r] is negative
+ *                or above INT32_MAX is invalid input here (a row's string is at most 2^31 - 1 bytes):
+ *                it reads as null and its bytes are never read.  Offsets are non-decreasing otherwise,
+ *                as Arrow requires.
  *  string_view / binary_view : validity | 16-byte views | var_data = gdv_view_buffers_t* (below)
  * `offset` is ArrayData::offset (in elements/bits), applied to every buffer.
  * validity may be NULL (no nulls). */
@@ -221,7 +233,8 @@ typedef struct gdv_batch {
 /* Caller-allocated output array (Projector::Evaluate allocates these from the
  * MemoryPool in the C++ layer).  Output offset is always 0.
  *  validity : ceil(n/8) bytes rounded up to 8; may be NULL -> validity not written
- *  values   : n*width bytes (bool: ceil(n/8) rounded up to 8); utf8: (n+1) int32 offsets
+ *  values   : n*width bytes (bool: ceil(n/8) rounded up to 8); utf8: (n+1) int32 offsets;
+ *             large_string / large_binary: (n+1) int64 offsets (no 2^31 - 1 byte limit)
  *  var_data : utf8/binary outputs only, capacity var_capacity bytes */
 typedef struct gdv_out_column {
   void* validity;
@@ -247,7 +260,8 @@ typedef struct gdv_selection {
                          use c = min(*d_num_slots, num_slots) rows.  Rows past c are not written: no
                          value, no offset past offsets[c], no byte past offsets[c], no validity word that
                          lies wholly past c (in the word holding row c-1 the bits past it are 0).
-                         utf8/binary outputs: values holds num_slots + 1 int32 offsets and var_data
+                         utf8/binary outputs: values holds num_slots + 1 int32 offsets (int64 for
+                         large_string / large_binary) and var_data
                          var_capacity bytes, an upper bound the caller picks; the byte total is
                          offsets[c].  var_size is the total after a synchronous call, -1 after an async
                          one.  A total above var_capacity is an ExecutionError (from the call when it is
