@@ -72,7 +72,7 @@ DataTypePtr FromC(const gdv_type_t& t) {
     case GDV_TYPE_DATE64: return arrow::date64();
     case GDV_TYPE_TIMESTAMP: return arrow::timestamp(static_cast<arrow::TimeUnit::type>(t.precision));
     case GDV_TYPE_TIME32: return arrow::time32(static_cast<arrow::TimeUnit::type>(t.precision));
-    case GDV_TYPE_TIME64: return arrow::time64(arrow::TimeUnit::MICRO);
+    case GDV_TYPE_TIME64: return arrow::time64(static_cast<arrow::TimeUnit::type>(t.precision));
     case GDV_TYPE_DECIMAL128: return arrow::decimal128(t.precision > 0 ? t.precision : 38, t.scale);
     default: return arrow::null();
   }

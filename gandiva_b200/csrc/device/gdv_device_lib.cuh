@@ -903,6 +903,12 @@ GDV_RELOP(i32, date32)
 GDV_RELOP(i64, date64)
 GDV_RELOP(i64, timestamp)
 GDV_RELOP(i32, time32)
+GDV_RELOP(i32, time32_s)
+GDV_RELOP(i64, timestamp_s)
+GDV_RELOP(i64, timestamp_us)
+GDV_RELOP(i64, timestamp_ns)
+GDV_RELOP(i64, time64_us)
+GDV_RELOP(i64, time64_ns)
 GDV_DEV bool equal_boolean_boolean(bool a, bool b) { return a == b; }
 GDV_DEV bool not_equal_boolean_boolean(bool a, bool b) { return a != b; }
 GDV_DEV bool not_boolean(bool a) { return !a; }
@@ -952,6 +958,12 @@ GDV_NULLTEST(i32, date32)
 GDV_NULLTEST(i64, date64)
 GDV_NULLTEST(i64, timestamp)
 GDV_NULLTEST(i32, time32)
+GDV_NULLTEST(i32, time32_s)
+GDV_NULLTEST(i64, timestamp_s)
+GDV_NULLTEST(i64, timestamp_us)
+GDV_NULLTEST(i64, timestamp_ns)
+GDV_NULLTEST(i64, time64_us)
+GDV_NULLTEST(i64, time64_ns)
 GDV_NULLTEST(bool, boolean)
 GDV_NULLTEST(i128, decimal128)
 GDV_NULLTEST(gdv_str, utf8)
@@ -983,6 +995,12 @@ GDV_DISTINCT(i32, date32)
 GDV_DISTINCT(i64, date64)
 GDV_DISTINCT(i64, timestamp)
 GDV_DISTINCT(i32, time32)
+GDV_DISTINCT(i32, time32_s)
+GDV_DISTINCT(i64, timestamp_s)
+GDV_DISTINCT(i64, timestamp_us)
+GDV_DISTINCT(i64, timestamp_ns)
+GDV_DISTINCT(i64, time64_us)
+GDV_DISTINCT(i64, time64_ns)
 GDV_DISTINCT(bool, boolean)
 
 // ---- casts -----------------------------------------------------------------------------
@@ -1007,10 +1025,30 @@ GDV_DEV i64 gdv_floordiv(i64 a, i64 b) {
   if ((a % b != 0) && ((a < 0) != (b < 0))) --q;
   return q;
 }
-// days -> milliseconds with two's-complement wrap (dates within 86400 s of the int64 limits have
-// month / year starts outside the range: the result is then defined, and the oracle's, not UB)
-GDV_DEV i64 gdv_days_to_ms(i64 days) { return (i64)((u64)days * 86400000ull); }
-GDV_DEV i64 castDATE_timestamp(i64 ms) { return gdv_days_to_ms(gdv_floordiv(ms, 86400000ll)); }
+// ---- time units -----------------------------------------------------------------------------
+// A timestamp, date64 or time value is a count of ticks; TPS is the unit's ticks per second (1, 1000,
+// 1000000, 1000000000 for s, ms, us, ns).  Every temporal core below takes TPS as a template argument,
+// so each division by a unit reaches the compiler as a division by a constant (a multiply-high, never
+// the 64-bit division routine), and the millisecond functions are the TPS = 1000 instances.
+#define GDV_UNITS(X) X(s, 1ll) X(ms, 1000ll) X(us, 1000000ll) X(ns, 1000000000ll)
+template <i64 TPS> GDV_DEV i64 gdv_day_of(i64 t) { return gdv_floordiv(t, 86400ll * TPS); }
+// ticks since the start of the day, in [0, ticks per day): computed modulo 2^64, so it is exact even
+// where day * ticks-per-day lies outside int64 (the first and last day of the range)
+template <i64 TPS> GDV_DEV i64 gdv_tick_of_day(i64 t) {
+  return (i64)((u64)t - (u64)gdv_day_of<TPS>(t) * (u64)(86400ll * TPS));
+}
+// days -> ticks with two's-complement wrap (dates within a day of the int64 limits have month / year
+// starts outside the range: the result is then defined, and the oracle's, not UB)
+template <i64 TPS> GDV_DEV i64 gdv_days_to_ticks(i64 days) { return (i64)((u64)days * (u64)(86400ll * TPS)); }
+GDV_DEV i64 gdv_days_to_ms(i64 days) { return gdv_days_to_ticks<1000ll>(days); }
+// ticks of unit FROM -> ticks of unit TO: widening multiplies with wrap, narrowing floors toward -inf
+template <i64 FROM, i64 TO> GDV_DEV i64 gdv_convert_ticks(i64 t) {
+  if (FROM == TO) return t;
+  if (FROM < TO) return (i64)((u64)t * (u64)(FROM < TO ? TO / FROM : 1));
+  return gdv_floordiv(t, FROM > TO ? FROM / TO : 1);
+}
+template <i64 TPS> GDV_DEV i64 gdv_cast_date(i64 t) { return gdv_days_to_ms(gdv_day_of<TPS>(t)); }
+GDV_DEV i64 castDATE_timestamp(i64 ms) { return gdv_cast_date<1000ll>(ms); }
 
 // ---- date / time extraction (proleptic Gregorian, days-from-civil inverse) ---------------
 struct gdv_ymd {
@@ -1034,40 +1072,28 @@ GDV_DEV gdv_ymd gdv_civil_from_days(i64 z) {
   r.doy = cum[r.m - 1] + r.d + ((leap && r.m > 2) ? 1 : 0);
   return r;
 }
-#define GDV_EXTRACT_MS(S)                                                                       \
-  GDV_DEV i64 extractYear_##S(i64 ms) {                                                         \
-    return gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).y;                                 \
-  }                                                                                             \
-  GDV_DEV i64 extractMonth_##S(i64 ms) {                                                        \
-    return gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).m;                                 \
-  }                                                                                             \
-  GDV_DEV i64 extractDay_##S(i64 ms) {                                                          \
-    return gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).d;                                 \
-  }                                                                                             \
-  GDV_DEV i64 extractDoy_##S(i64 ms) {                                                          \
-    return gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).doy;                               \
-  }                                                                                             \
-  GDV_DEV i64 extractQuarter_##S(i64 ms) {                                                      \
-    return (gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).m - 1) / 3 + 1;                   \
-  }                                                                                             \
-  GDV_DEV i64 extractDow_##S(i64 ms) {                                                          \
-    const i64 days = gdv_floordiv(ms, 86400000ll);                                              \
-    i64 w = (days + 4) % 7; /* 1970-01-01 was a Thursday; Sunday = 1 */                         \
-    if (w < 0) w += 7;                                                                          \
-    return w + 1;                                                                               \
-  }                                                                                             \
-  GDV_DEV i64 extractHour_##S(i64 ms) {                                                         \
-    return (ms - gdv_floordiv(ms, 86400000ll) * 86400000ll) / 3600000ll;                        \
-  }                                                                                             \
-  GDV_DEV i64 extractMinute_##S(i64 ms) {                                                       \
-    return ((ms - gdv_floordiv(ms, 86400000ll) * 86400000ll) / 60000ll) % 60;                   \
-  }                                                                                             \
-  GDV_DEV i64 extractSecond_##S(i64 ms) {                                                       \
-    return ((ms - gdv_floordiv(ms, 86400000ll) * 86400000ll) / 1000ll) % 60;                    \
-  }                                                                                             \
-  GDV_DEV i64 extractEpoch_##S(i64 ms) { return gdv_floordiv(ms, 1000ll); }
-GDV_EXTRACT_MS(date64)
-GDV_EXTRACT_MS(timestamp)
+// calendar fields of floor(ticks / ticks per day) and the time of day, at any unit
+#define GDV_EXTRACT(S, TPS)                                                                        \
+  GDV_DEV i64 extractYear_##S(i64 t) { return gdv_civil_from_days(gdv_day_of<TPS>(t)).y; }         \
+  GDV_DEV i64 extractMonth_##S(i64 t) { return gdv_civil_from_days(gdv_day_of<TPS>(t)).m; }        \
+  GDV_DEV i64 extractDay_##S(i64 t) { return gdv_civil_from_days(gdv_day_of<TPS>(t)).d; }          \
+  GDV_DEV i64 extractDoy_##S(i64 t) { return gdv_civil_from_days(gdv_day_of<TPS>(t)).doy; }        \
+  GDV_DEV i64 extractQuarter_##S(i64 t) { return (gdv_civil_from_days(gdv_day_of<TPS>(t)).m - 1) / 3 + 1; } \
+  GDV_DEV i64 extractDow_##S(i64 t) {                                                              \
+    const i64 days = gdv_day_of<TPS>(t);                                                           \
+    i64 w = (days + 4) % 7; /* 1970-01-01 was a Thursday; Sunday = 1 */                            \
+    if (w < 0) w += 7;                                                                             \
+    return w + 1;                                                                                  \
+  }                                                                                                \
+  GDV_DEV i64 extractHour_##S(i64 t) { return gdv_tick_of_day<TPS>(t) / (3600ll * TPS); }          \
+  GDV_DEV i64 extractMinute_##S(i64 t) { return (gdv_tick_of_day<TPS>(t) / (60ll * TPS)) % 60; }   \
+  GDV_DEV i64 extractSecond_##S(i64 t) { return (gdv_tick_of_day<TPS>(t) / TPS) % 60; }            \
+  GDV_DEV i64 extractEpoch_##S(i64 t) { return gdv_floordiv(t, TPS); }
+GDV_EXTRACT(date64, 1000ll)
+GDV_EXTRACT(timestamp, 1000ll)
+GDV_EXTRACT(timestamp_s, 1ll)
+GDV_EXTRACT(timestamp_us, 1000000ll)
+GDV_EXTRACT(timestamp_ns, 1000000000ll)
 GDV_DEV i64 extractYear_date32(i32 d) { return gdv_civil_from_days((i64)d).y; }
 GDV_DEV i64 extractMonth_date32(i32 d) { return gdv_civil_from_days((i64)d).m; }
 GDV_DEV i64 extractDay_date32(i32 d) { return gdv_civil_from_days((i64)d).d; }
@@ -1148,10 +1174,10 @@ GDV_DEV i64 gdv_days_from_civil(i64 y, i32 m, i32 d) {
   return era * 146097 + doe - 719468;
 }
 // Calendar month arithmetic: the day of month is clamped to the length of the target month
-// (Jan 31 + 1 month = Feb 28/29); the time of day is kept.
-GDV_DEV i64 gdv_add_months(i64 ms, i64 months) {
-  const i64 days = gdv_floordiv(ms, 86400000ll);
-  const i64 in_day = ms - days * 86400000ll;
+// (Jan 31 + 1 month = Feb 28/29); the time of day, to the tick, is kept.
+template <i64 TPS> GDV_DEV i64 gdv_add_months_u(i64 t, i64 months) {
+  const i64 days = gdv_day_of<TPS>(t);
+  const i64 in_day = gdv_tick_of_day<TPS>(t);
   const gdv_ymd c = gdv_civil_from_days(days);
   const i64 total = c.y * 12 + (i64)(c.m - 1) + months;
   const i64 ny = gdv_floordiv(total, 12);
@@ -1159,80 +1185,92 @@ GDV_DEV i64 gdv_add_months(i64 ms, i64 months) {
   const bool leap = (ny % 4 == 0) && ((ny % 100 != 0) || (ny % 400 == 0));
   const i32 mlen[12] = {31, leap ? 29 : 28, 31, 30, 31, 30, 31, 31, 30, 31, 30, 31};
   const i32 nd = c.d < mlen[nm - 1] ? c.d : mlen[nm - 1];
-  return (i64)((u64)gdv_days_to_ms(gdv_days_from_civil(ny, nm, nd)) + (u64)in_day);
+  return (i64)((u64)gdv_days_to_ticks<TPS>(gdv_days_from_civil(ny, nm, nd)) + (u64)in_day);
 }
-#define GDV_TSADD(NAME, UNIT_MS)                                                                  \
-  GDV_DEV i64 NAME##_int32_timestamp(i32 n, i64 ts) { return (i64)((u64)ts + (u64)((i64)n * (UNIT_MS))); } \
-  GDV_DEV i64 NAME##_int64_timestamp(i64 n, i64 ts) { return (i64)((u64)ts + (u64)n * (u64)(UNIT_MS)); } \
-  GDV_DEV i64 NAME##_timestamp_int32(i64 ts, i32 n) { return NAME##_int32_timestamp(n, ts); }     \
-  GDV_DEV i64 NAME##_timestamp_int64(i64 ts, i64 n) { return NAME##_int64_timestamp(n, ts); }
-GDV_TSADD(timestampaddSecond, 1000ll)
-GDV_TSADD(timestampaddMinute, 60000ll)
-GDV_TSADD(timestampaddHour, 3600000ll)
-GDV_TSADD(timestampaddDay, 86400000ll)
-GDV_TSADD(timestampaddWeek, 604800000ll)
-// calendar units: month counts wrap in 64 bits (an int64 count times 3 or 12), like the millisecond units
-#define GDV_TSADD_MONTHS(NAME, K)                                                                 \
-  GDV_DEV i64 NAME##_int32_timestamp(i32 n, i64 ts) { return gdv_add_months(ts, (K) * (i64)n); }  \
-  GDV_DEV i64 NAME##_int64_timestamp(i64 n, i64 ts) { return gdv_add_months(ts, (i64)((u64)(K) * (u64)n)); } \
-  GDV_DEV i64 NAME##_timestamp_int32(i64 ts, i32 n) { return NAME##_int32_timestamp(n, ts); }     \
-  GDV_DEV i64 NAME##_timestamp_int64(i64 ts, i64 n) { return NAME##_int64_timestamp(n, ts); }
-GDV_TSADD_MONTHS(timestampaddMonth, 1ll)
-GDV_TSADD_MONTHS(timestampaddQuarter, 3ll)
-GDV_TSADD_MONTHS(timestampaddYear, 12ll)
-// add_months(date | timestamp, n): timestampaddMonth with the arguments the other way round
-GDV_DEV i64 add_months_date64_int32(i64 d, i32 n) { return gdv_add_months(d, (i64)n); }
-GDV_DEV i64 add_months_date64_int64(i64 d, i64 n) { return gdv_add_months(d, n); }
-GDV_DEV i64 add_months_timestamp_int32(i64 d, i32 n) { return gdv_add_months(d, (i64)n); }
-GDV_DEV i64 add_months_timestamp_int64(i64 d, i64 n) { return gdv_add_months(d, n); }
-GDV_DEV i64 date_add_date64_int32(i64 d, i32 n) { return (i64)((u64)d + (u64)((i64)n * 86400000ll)); }
-GDV_DEV i64 date_sub_date64_int32(i64 d, i32 n) { return (i64)((u64)d - (u64)((i64)n * 86400000ll)); }
-GDV_DEV i64 date_add_timestamp_int32(i64 d, i32 n) { return date_add_date64_int32(d, n); }
-GDV_DEV i64 date_sub_timestamp_int32(i64 d, i32 n) { return date_sub_date64_int32(d, n); }
-#define GDV_TSDIFF(NAME, UNIT_MS)                                                                 \
-  GDV_DEV i32 NAME##_timestamp_timestamp(i64 a, i64 b) {                                          \
-    return (i32)(u32)(u64)((i64)((u64)b - (u64)a) / (UNIT_MS));                                   \
+GDV_DEV i64 gdv_add_months(i64 ms, i64 months) { return gdv_add_months_u<1000ll>(ms, months); }
+// fixed-length steps: count * ticks per step, added with int64 wrap
+#define GDV_TSADD(NAME, SECS, S, TPS)                                                             \
+  GDV_DEV i64 NAME##_int32_##S(i32 n, i64 ts) { return (i64)((u64)ts + (u64)(i64)n * (u64)((SECS) * TPS)); } \
+  GDV_DEV i64 NAME##_int64_##S(i64 n, i64 ts) { return (i64)((u64)ts + (u64)n * (u64)((SECS) * TPS)); } \
+  GDV_DEV i64 NAME##_##S##_int32(i64 ts, i32 n) { return NAME##_int32_##S(n, ts); }               \
+  GDV_DEV i64 NAME##_##S##_int64(i64 ts, i64 n) { return NAME##_int64_##S(n, ts); }
+// calendar units: month counts wrap in 64 bits (an int64 count times 3 or 12), like the fixed steps
+#define GDV_TSADD_MONTHS(NAME, K, S, TPS)                                                          \
+  GDV_DEV i64 NAME##_int32_##S(i32 n, i64 ts) { return gdv_add_months_u<TPS>(ts, (K) * (i64)n); } \
+  GDV_DEV i64 NAME##_int64_##S(i64 n, i64 ts) { return gdv_add_months_u<TPS>(ts, (i64)((u64)(K) * (u64)n)); } \
+  GDV_DEV i64 NAME##_##S##_int32(i64 ts, i32 n) { return NAME##_int32_##S(n, ts); }               \
+  GDV_DEV i64 NAME##_##S##_int64(i64 ts, i64 n) { return NAME##_int64_##S(n, ts); }
+// timestampdiff{Second..Week}(a, b): (b - a) / ticks per step, truncated, the difference wrapping in int64
+#define GDV_TSDIFF(NAME, SECS, S, TPS)                                                            \
+  GDV_DEV i32 NAME##_##S##_##S(i64 a, i64 b) {                                                    \
+    return (i32)(u32)(u64)((i64)((u64)b - (u64)a) / ((SECS) * TPS));                              \
   }
-GDV_TSDIFF(timestampdiffSecond, 1000ll)
-GDV_TSDIFF(timestampdiffMinute, 60000ll)
-GDV_TSDIFF(timestampdiffHour, 3600000ll)
-GDV_TSDIFF(timestampdiffDay, 86400000ll)
-GDV_TSDIFF(timestampdiffWeek, 604800000ll)
 
 // timestampdiff{Month,Quarter,Year}(a, b): whole calendar months from a to b, consistent with
 // timestampaddMonth: the largest |k| such that a + k months (day clamped to the month's length,
 // time of day kept) does not pass b; quarters and years are that count / 3 and / 12, truncated.
-GDV_DEV_BIG i64 gdv_months_between_whole(i64 a, i64 b) {
-  const gdv_ymd ca = gdv_civil_from_days(gdv_floordiv(a, 86400000ll));
-  const gdv_ymd cb = gdv_civil_from_days(gdv_floordiv(b, 86400000ll));
+template <i64 TPS> GDV_DEV_BIG i64 gdv_months_between_whole(i64 a, i64 b) {
+  const gdv_ymd ca = gdv_civil_from_days(gdv_day_of<TPS>(a));
+  const gdv_ymd cb = gdv_civil_from_days(gdv_day_of<TPS>(b));
   i64 k = (cb.y - ca.y) * 12 + (i64)(cb.m - ca.m);
   if (b >= a) {
-    if (k > 0 && gdv_add_months(a, k) > b) --k;
+    if (k > 0 && gdv_add_months_u<TPS>(a, k) > b) --k;
     if (k < 0) k = 0;
   } else {
-    if (k < 0 && gdv_add_months(a, k) < b) ++k;
+    if (k < 0 && gdv_add_months_u<TPS>(a, k) < b) ++k;
     if (k > 0) k = 0;
   }
   return k;
 }
-GDV_DEV i32 timestampdiffMonth_timestamp_timestamp(i64 a, i64 b) { return (i32)gdv_months_between_whole(a, b); }
-GDV_DEV i32 timestampdiffQuarter_timestamp_timestamp(i64 a, i64 b) { return (i32)(gdv_months_between_whole(a, b) / 3); }
-GDV_DEV i32 timestampdiffYear_timestamp_timestamp(i64 a, i64 b) { return (i32)(gdv_months_between_whole(a, b) / 12); }
 // months_between(a, b) (Hive / Oracle): a - b in months; whole when both are the same day of the
 // month or both the last day of theirs, else the month difference plus (day and time of day
-// difference) / 31 days; IEEE double operations in a fixed order.
-GDV_DEV_BIG f64 gdv_months_between(i64 a, i64 b) {
-  const i64 da = gdv_floordiv(a, 86400000ll), db = gdv_floordiv(b, 86400000ll);
+// difference) / 31 days; IEEE double operations in a fixed order.  The time-of-day difference is
+// exact in a double at every unit, so ms-aligned ticks give the millisecond result bit for bit.
+template <i64 TPS> GDV_DEV_BIG f64 gdv_months_between(i64 a, i64 b) {
+  const i64 da = gdv_day_of<TPS>(a), db = gdv_day_of<TPS>(b);
   const gdv_ymd ca = gdv_civil_from_days(da), cb = gdv_civil_from_days(db);
   const f64 months = (f64)((ca.y - cb.y) * 12 + (i64)(ca.m - cb.m));
   const bool last_a = gdv_civil_from_days(da + 1).d == 1, last_b = gdv_civil_from_days(db + 1).d == 1;
   if (ca.d == cb.d || (last_a && last_b)) return months;
-  const i64 ta = a - da * 86400000ll, tb = b - db * 86400000ll;
-  const f64 secs = (f64)((i64)(ca.d - cb.d) * 86400ll) + (f64)(ta - tb) / 1000.0;
+  const i64 ta = gdv_tick_of_day<TPS>(a), tb = gdv_tick_of_day<TPS>(b);
+  const f64 secs = (f64)((i64)(ca.d - cb.d) * 86400ll) + (f64)(ta - tb) / (f64)TPS;
   return months + secs / 2678400.0;
 }
-GDV_DEV f64 months_between_timestamp_timestamp(i64 a, i64 b) { return gdv_months_between(a, b); }
-GDV_DEV f64 months_between_date64_date64(i64 a, i64 b) { return gdv_months_between(a, b); }
+// The timestamp arithmetic family of one unit (S = the type's suffix).  add_months(timestamp, n) is
+// timestampaddMonth with the arguments the other way round; date_add / date_sub step whole days.
+#define GDV_TS_ARITH(S, TPS)                                                                      \
+  GDV_TSADD(timestampaddSecond, 1ll, S, TPS)                                                      \
+  GDV_TSADD(timestampaddMinute, 60ll, S, TPS)                                                     \
+  GDV_TSADD(timestampaddHour, 3600ll, S, TPS)                                                     \
+  GDV_TSADD(timestampaddDay, 86400ll, S, TPS)                                                     \
+  GDV_TSADD(timestampaddWeek, 604800ll, S, TPS)                                                   \
+  GDV_TSADD_MONTHS(timestampaddMonth, 1ll, S, TPS)                                                \
+  GDV_TSADD_MONTHS(timestampaddQuarter, 3ll, S, TPS)                                              \
+  GDV_TSADD_MONTHS(timestampaddYear, 12ll, S, TPS)                                                \
+  GDV_DEV i64 add_months_##S##_int32(i64 d, i32 n) { return gdv_add_months_u<TPS>(d, (i64)n); }   \
+  GDV_DEV i64 add_months_##S##_int64(i64 d, i64 n) { return gdv_add_months_u<TPS>(d, n); }        \
+  GDV_DEV i64 date_add_##S##_int32(i64 d, i32 n) { return (i64)((u64)d + (u64)(i64)n * (u64)(86400ll * TPS)); } \
+  GDV_DEV i64 date_sub_##S##_int32(i64 d, i32 n) { return (i64)((u64)d - (u64)(i64)n * (u64)(86400ll * TPS)); } \
+  GDV_TSDIFF(timestampdiffSecond, 1ll, S, TPS)                                                    \
+  GDV_TSDIFF(timestampdiffMinute, 60ll, S, TPS)                                                   \
+  GDV_TSDIFF(timestampdiffHour, 3600ll, S, TPS)                                                   \
+  GDV_TSDIFF(timestampdiffDay, 86400ll, S, TPS)                                                   \
+  GDV_TSDIFF(timestampdiffWeek, 604800ll, S, TPS)                                                 \
+  GDV_DEV i32 timestampdiffMonth_##S##_##S(i64 a, i64 b) { return (i32)gdv_months_between_whole<TPS>(a, b); } \
+  GDV_DEV i32 timestampdiffQuarter_##S##_##S(i64 a, i64 b) { return (i32)(gdv_months_between_whole<TPS>(a, b) / 3); } \
+  GDV_DEV i32 timestampdiffYear_##S##_##S(i64 a, i64 b) { return (i32)(gdv_months_between_whole<TPS>(a, b) / 12); } \
+  GDV_DEV f64 months_between_##S##_##S(i64 a, i64 b) { return gdv_months_between<TPS>(a, b); }   \
+  GDV_DEV i32 datediff_##S##_##S(i64 a, i64 b) { return (i32)(gdv_day_of<TPS>(a) - gdv_day_of<TPS>(b)); }
+GDV_TS_ARITH(timestamp, 1000ll)
+GDV_TS_ARITH(timestamp_s, 1ll)
+GDV_TS_ARITH(timestamp_us, 1000000ll)
+GDV_TS_ARITH(timestamp_ns, 1000000000ll)
+GDV_DEV i64 add_months_date64_int32(i64 d, i32 n) { return gdv_add_months(d, (i64)n); }
+GDV_DEV i64 add_months_date64_int64(i64 d, i64 n) { return gdv_add_months(d, n); }
+GDV_DEV i64 date_add_date64_int32(i64 d, i32 n) { return date_add_timestamp_int32(d, n); }
+GDV_DEV i64 date_sub_date64_int32(i64 d, i32 n) { return date_sub_timestamp_int32(d, n); }
+GDV_DEV f64 months_between_date64_date64(i64 a, i64 b) { return gdv_months_between<1000ll>(a, b); }
+GDV_DEV i32 datediff_date64_date64(i64 a, i64 b) { return datediff_timestamp_timestamp(a, b); }
 
 // ---- calendar fields and truncation -------------------------------------------------------------
 // ISO 8601 week of the year (weeks start on Monday, week 1 holds the year's first Thursday).
@@ -1259,52 +1297,56 @@ GDV_DEV i64 gdv_iso_week(i64 days) {
 }
 // date_trunc: the first instant of the enclosing unit; weeks start on Monday; decades start in
 // years divisible by 10, centuries / millennia in years ...01 (C truncating division on the year).
-GDV_DEV i64 gdv_trunc_year_to(i64 ms, i64 span, i64 first) {
-  const gdv_ymd c = gdv_civil_from_days(gdv_floordiv(ms, 86400000ll));
+template <i64 TPS> GDV_DEV i64 gdv_trunc_year_to(i64 t, i64 span, i64 first) {
+  const gdv_ymd c = gdv_civil_from_days(gdv_day_of<TPS>(t));
   const i64 y = span == 10 ? (c.y / 10) * 10 : ((c.y - 1) / span) * span + first;
-  return gdv_days_to_ms(gdv_days_from_civil(span == 1 ? c.y : y, 1, 1));
+  return gdv_days_to_ticks<TPS>(gdv_days_from_civil(span == 1 ? c.y : y, 1, 1));
 }
-#define GDV_CALENDAR(S)                                                                           \
-  GDV_DEV i64 extractWeek_##S(i64 ms) { return gdv_iso_week(gdv_floordiv(ms, 86400000ll)); }      \
-  GDV_DEV i64 extractDecade_##S(i64 ms) {                                                         \
-    return gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).y / 10;                              \
+// floor to a multiple of STEP ticks (wraps like the day-based truncations below the int64 minimum)
+template <i64 STEP> GDV_DEV i64 gdv_floor_to(i64 t) { return (i64)((u64)gdv_floordiv(t, STEP) * (u64)STEP); }
+// The results of date_trunc_* are in the argument's unit; last_day is a date64 (milliseconds).
+#define GDV_CALENDAR(S, TPS)                                                                      \
+  GDV_DEV i64 extractWeek_##S(i64 t) { return gdv_iso_week(gdv_day_of<TPS>(t)); }                 \
+  GDV_DEV i64 extractDecade_##S(i64 t) { return gdv_civil_from_days(gdv_day_of<TPS>(t)).y / 10; } \
+  GDV_DEV i64 extractCentury_##S(i64 t) {                                                         \
+    return (gdv_civil_from_days(gdv_day_of<TPS>(t)).y - 1) / 100 + 1;                             \
   }                                                                                               \
-  GDV_DEV i64 extractCentury_##S(i64 ms) {                                                        \
-    return (gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).y - 1) / 100 + 1;                   \
+  GDV_DEV i64 extractMillennium_##S(i64 t) {                                                      \
+    return (gdv_civil_from_days(gdv_day_of<TPS>(t)).y - 1) / 1000 + 1;                            \
   }                                                                                               \
-  GDV_DEV i64 extractMillennium_##S(i64 ms) {                                                     \
-    return (gdv_civil_from_days(gdv_floordiv(ms, 86400000ll)).y - 1) / 1000 + 1;                  \
-  }                                                                                               \
-  GDV_DEV i64 date_trunc_Second_##S(i64 ms) { return gdv_floordiv(ms, 1000ll) * 1000ll; }         \
-  GDV_DEV i64 date_trunc_Minute_##S(i64 ms) { return gdv_floordiv(ms, 60000ll) * 60000ll; }       \
-  GDV_DEV i64 date_trunc_Hour_##S(i64 ms) { return gdv_floordiv(ms, 3600000ll) * 3600000ll; }     \
-  GDV_DEV i64 date_trunc_Day_##S(i64 ms) { return gdv_days_to_ms(gdv_floordiv(ms, 86400000ll)); } \
-  GDV_DEV i64 date_trunc_Week_##S(i64 ms) {                                                       \
-    const i64 days = gdv_floordiv(ms, 86400000ll);                                                \
+  GDV_DEV i64 date_trunc_Second_##S(i64 t) { return gdv_floor_to<TPS>(t); }                       \
+  GDV_DEV i64 date_trunc_Minute_##S(i64 t) { return gdv_floor_to<60ll * TPS>(t); }                \
+  GDV_DEV i64 date_trunc_Hour_##S(i64 t) { return gdv_floor_to<3600ll * TPS>(t); }                \
+  GDV_DEV i64 date_trunc_Day_##S(i64 t) { return gdv_days_to_ticks<TPS>(gdv_day_of<TPS>(t)); }    \
+  GDV_DEV i64 date_trunc_Week_##S(i64 t) {                                                        \
+    const i64 days = gdv_day_of<TPS>(t);                                                          \
     i64 wd = (days + 3) % 7;                                                                      \
     if (wd < 0) wd += 7;                                                                          \
-    return gdv_days_to_ms(days - wd);                                                             \
+    return gdv_days_to_ticks<TPS>(days - wd);                                                     \
   }                                                                                               \
-  GDV_DEV i64 date_trunc_Month_##S(i64 ms) {                                                      \
-    const gdv_ymd c = gdv_civil_from_days(gdv_floordiv(ms, 86400000ll));                          \
-    return gdv_days_to_ms(gdv_days_from_civil(c.y, c.m, 1));                                      \
+  GDV_DEV i64 date_trunc_Month_##S(i64 t) {                                                       \
+    const gdv_ymd c = gdv_civil_from_days(gdv_day_of<TPS>(t));                                    \
+    return gdv_days_to_ticks<TPS>(gdv_days_from_civil(c.y, c.m, 1));                              \
   }                                                                                               \
-  GDV_DEV i64 date_trunc_Quarter_##S(i64 ms) {                                                    \
-    const gdv_ymd c = gdv_civil_from_days(gdv_floordiv(ms, 86400000ll));                          \
-    return gdv_days_to_ms(gdv_days_from_civil(c.y, ((c.m - 1) / 3) * 3 + 1, 1));                  \
+  GDV_DEV i64 date_trunc_Quarter_##S(i64 t) {                                                     \
+    const gdv_ymd c = gdv_civil_from_days(gdv_day_of<TPS>(t));                                    \
+    return gdv_days_to_ticks<TPS>(gdv_days_from_civil(c.y, ((c.m - 1) / 3) * 3 + 1, 1));          \
   }                                                                                               \
-  GDV_DEV i64 date_trunc_Year_##S(i64 ms) { return gdv_trunc_year_to(ms, 1, 0); }                 \
-  GDV_DEV i64 date_trunc_Decade_##S(i64 ms) { return gdv_trunc_year_to(ms, 10, 0); }              \
-  GDV_DEV i64 date_trunc_Century_##S(i64 ms) { return gdv_trunc_year_to(ms, 100, 1); }            \
-  GDV_DEV i64 date_trunc_Millennium_##S(i64 ms) { return gdv_trunc_year_to(ms, 1000, 1); }        \
-  GDV_DEV i64 last_day_##S(i64 ms) {                                                              \
-    const gdv_ymd c = gdv_civil_from_days(gdv_floordiv(ms, 86400000ll));                          \
+  GDV_DEV i64 date_trunc_Year_##S(i64 t) { return gdv_trunc_year_to<TPS>(t, 1, 0); }              \
+  GDV_DEV i64 date_trunc_Decade_##S(i64 t) { return gdv_trunc_year_to<TPS>(t, 10, 0); }           \
+  GDV_DEV i64 date_trunc_Century_##S(i64 t) { return gdv_trunc_year_to<TPS>(t, 100, 1); }         \
+  GDV_DEV i64 date_trunc_Millennium_##S(i64 t) { return gdv_trunc_year_to<TPS>(t, 1000, 1); }     \
+  GDV_DEV i64 last_day_##S(i64 t) {                                                               \
+    const gdv_ymd c = gdv_civil_from_days(gdv_day_of<TPS>(t));                                    \
     const i64 ny = c.m == 12 ? c.y + 1 : c.y;                                                     \
     const i32 nm = c.m == 12 ? 1 : c.m + 1;                                                       \
     return gdv_days_to_ms(gdv_days_from_civil(ny, nm, 1) - 1);                                    \
   }
-GDV_CALENDAR(date64)
-GDV_CALENDAR(timestamp)
+GDV_CALENDAR(date64, 1000ll)
+GDV_CALENDAR(timestamp, 1000ll)
+GDV_CALENDAR(timestamp_s, 1ll)
+GDV_CALENDAR(timestamp_us, 1000000ll)
+GDV_CALENDAR(timestamp_ns, 1000000000ll)
 // float -> integer casts: round half away from zero, then saturate at the ends of the type; NaN -> 0
 GDV_DEV i64 castBIGINT_float64(f64 x) {
   if (x != x) return 0ll;
@@ -1322,22 +1364,57 @@ GDV_DEV i32 castINT_float64(f64 x) {
   return (i32)r;
 }
 GDV_DEV i32 castINT_float32(f32 x) { return castINT_float64((f64)x); }
-// to_timestamp(seconds since the epoch) / to_time(seconds): milliseconds, fractions truncated toward
-// zero; to_time keeps the time of day in [0, 86 400 000)
-GDV_DEV i64 to_timestamp_int64(i64 sec) { return (i64)((u64)sec * 1000ull); }
-GDV_DEV i64 to_timestamp_int32(i32 sec) { return (i64)sec * 1000ll; }
-GDV_DEV i64 to_timestamp_float64(f64 sec) { return castBIGINT_float64(trunc(sec * 1000.0)); }
+// to_timestamp(seconds since the epoch) / to_time(seconds) in the declared unit: whole seconds times
+// ticks per second with int64 wrap, fractions (seconds * ticks per second) truncated toward zero;
+// to_time keeps the time of day in [0, ticks per day)
+template <i64 TPS> GDV_DEV i64 gdv_to_timestamp(i64 sec) { return (i64)((u64)sec * (u64)TPS); }
+template <i64 TPS> GDV_DEV i64 gdv_to_timestamp_f(f64 sec) { return castBIGINT_float64(trunc(sec * (f64)TPS)); }
+GDV_DEV i64 to_timestamp_int64(i64 sec) { return gdv_to_timestamp<1000ll>(sec); }
+GDV_DEV i64 to_timestamp_int32(i32 sec) { return gdv_to_timestamp<1000ll>((i64)sec); }
+GDV_DEV i64 to_timestamp_float64(f64 sec) { return gdv_to_timestamp_f<1000ll>(sec); }
 GDV_DEV i64 to_timestamp_float32(f32 sec) { return to_timestamp_float64((f64)sec); }
-GDV_DEV i32 gdv_ms_of_day(i64 ms) { return (i32)(ms - gdv_floordiv(ms, 86400000ll) * 86400000ll); }
+GDV_DEV i32 gdv_ms_of_day(i64 ms) { return (i32)gdv_tick_of_day<1000ll>(ms); }
 GDV_DEV i32 to_time_int64(i64 sec) { return gdv_ms_of_day(to_timestamp_int64(sec)); }
 GDV_DEV i32 to_time_int32(i32 sec) { return gdv_ms_of_day(to_timestamp_int32(sec)); }
 GDV_DEV i32 to_time_float64(f64 sec) { return gdv_ms_of_day(to_timestamp_float64(sec)); }
 GDV_DEV i32 to_time_float32(f32 sec) { return gdv_ms_of_day(to_timestamp_float64((f64)sec)); }
 // time of day (time32[ms]) of a timestamp, and its fields
-GDV_DEV i32 castTIME_timestamp(i64 ms) { return (i32)(ms - gdv_floordiv(ms, 86400000ll) * 86400000ll); }
-GDV_DEV i64 extractHour_time32(i32 t) { return (i64)(t / 3600000); }
-GDV_DEV i64 extractMinute_time32(i32 t) { return (i64)((t / 60000) % 60); }
-GDV_DEV i64 extractSecond_time32(i32 t) { return (i64)((t / 1000) % 60); }
+GDV_DEV i32 castTIME_timestamp(i64 ms) { return gdv_ms_of_day(ms); }
+#define GDV_TIME_FIELDS(T, S, TPS)                                                                \
+  GDV_DEV i64 extractHour_##S(T t) { return (i64)(t / (T)(3600ll * TPS)); }                       \
+  GDV_DEV i64 extractMinute_##S(T t) { return (i64)((t / (T)(60ll * TPS)) % 60); }                \
+  GDV_DEV i64 extractSecond_##S(T t) { return (i64)((t / (T)TPS) % 60); }
+GDV_TIME_FIELDS(i32, time32, 1000ll)
+GDV_TIME_FIELDS(i32, time32_s, 1ll)
+GDV_TIME_FIELDS(i64, time64_us, 1000000ll)
+GDV_TIME_FIELDS(i64, time64_ns, 1000000000ll)
+// The other units' constructors take the declared unit's name (to_timestamp_us_int64, ...); a time
+// of day is a time32 (i32) in s and ms and a time64 (i64) in us and ns.
+#define GDV_TIME_UNIT(U, TPS, TT, TS)                                                            \
+  GDV_DEV i64 to_timestamp_##U##_int64(i64 sec) { return gdv_to_timestamp<TPS>(sec); }            \
+  GDV_DEV i64 to_timestamp_##U##_int32(i32 sec) { return gdv_to_timestamp<TPS>((i64)sec); }       \
+  GDV_DEV i64 to_timestamp_##U##_float64(f64 sec) { return gdv_to_timestamp_f<TPS>(sec); }        \
+  GDV_DEV i64 to_timestamp_##U##_float32(f32 sec) { return gdv_to_timestamp_f<TPS>((f64)sec); }   \
+  GDV_DEV TT to_time_##U##_int64(i64 sec) { return (TT)gdv_tick_of_day<TPS>(gdv_to_timestamp<TPS>(sec)); } \
+  GDV_DEV TT to_time_##U##_int32(i32 sec) { return (TT)gdv_tick_of_day<TPS>(gdv_to_timestamp<TPS>((i64)sec)); } \
+  GDV_DEV TT to_time_##U##_float64(f64 sec) { return (TT)gdv_tick_of_day<TPS>(gdv_to_timestamp_f<TPS>(sec)); } \
+  GDV_DEV TT to_time_##U##_float32(f32 sec) { return (TT)gdv_tick_of_day<TPS>(gdv_to_timestamp_f<TPS>((f64)sec)); } \
+  GDV_DEV TT castTIME_##TS(i64 t) { return (TT)gdv_tick_of_day<TPS>(t); }                         \
+  GDV_DEV i64 castDATE_##TS(i64 t) { return gdv_cast_date<TPS>(t); }                              \
+  GDV_DEV i64 castBIGINT_##TS(i64 t) { return t; }                                                \
+  GDV_DEV i64 castTIMESTAMP_##U##_int64(i64 a) { return a; }                                      \
+  GDV_DEV i64 castTIMESTAMP_##U##_date64(i64 ms) { return gdv_convert_ticks<1000ll, TPS>(ms); }   \
+  GDV_DEV i64 castTIMESTAMP_##U##_timestamp_s(i64 t) { return gdv_convert_ticks<1ll, TPS>(t); }   \
+  GDV_DEV i64 castTIMESTAMP_##U##_timestamp(i64 t) { return gdv_convert_ticks<1000ll, TPS>(t); }  \
+  GDV_DEV i64 castTIMESTAMP_##U##_timestamp_us(i64 t) { return gdv_convert_ticks<1000000ll, TPS>(t); } \
+  GDV_DEV i64 castTIMESTAMP_##U##_timestamp_ns(i64 t) { return gdv_convert_ticks<1000000000ll, TPS>(t); }
+GDV_TIME_UNIT(s, 1ll, i32, timestamp_s)
+GDV_TIME_UNIT(us, 1000000ll, i64, timestamp_us)
+GDV_TIME_UNIT(ns, 1000000000ll, i64, timestamp_ns)
+// into milliseconds from the other units (the ms constructors above keep their plain names)
+GDV_DEV i64 castTIMESTAMP_ms_timestamp_s(i64 t) { return gdv_convert_ticks<1ll, 1000ll>(t); }
+GDV_DEV i64 castTIMESTAMP_ms_timestamp_us(i64 t) { return gdv_convert_ticks<1000000ll, 1000ll>(t); }
+GDV_DEV i64 castTIMESTAMP_ms_timestamp_ns(i64 t) { return gdv_convert_ticks<1000000000ll, 1000ll>(t); }
 
 // ---- decimal128 ------------------------------------------------------------------------
 // Values are two's-complement 128-bit integers scaled by 10^scale (Arrow decimal128).
@@ -2447,6 +2524,12 @@ GDV_HASH_NUM(i32, date32)
 GDV_HASH_NUM(i64, date64)
 GDV_HASH_NUM(i64, timestamp)
 GDV_HASH_NUM(i32, time32)
+GDV_HASH_NUM(i32, time32_s)
+GDV_HASH_NUM(i64, timestamp_s)
+GDV_HASH_NUM(i64, timestamp_us)
+GDV_HASH_NUM(i64, timestamp_ns)
+GDV_HASH_NUM(i64, time64_us)
+GDV_HASH_NUM(i64, time64_ns)
 #define GDV_HASH_STR(S)                                                                           \
   GDV_DEV i32 hash32_##S(gdv_str v, bool ok) { return ok ? (i32)gdv_murmur3_32_buf(v, 0) : 0; }   \
   GDV_DEV i32 hash32_##S##_int32(gdv_str v, bool ok, i32 seed, bool sok) {                        \
@@ -2800,7 +2883,8 @@ GDV_DEV i64 castBIGINT_utf8(gdv_ctx* c, gdv_str s) {
 GDV_DEV i32 castINT_utf8(gdv_ctx* c, gdv_str s) { return (i32)gdv_parse_int(c, s, -2147483648ll, 2147483647ll); }
 
 // castDATE / castTIMESTAMP of a string: [spaces] Y-M-D [(' ' | 'T') h:m[:s[.fraction]]] [spaces],
-// 1..9 digit year (optional leading '-'), 1..2 digit fields, fraction truncated to milliseconds;
+// 1..9 digit year (optional leading '-'), 1..2 digit fields, fraction truncated to the unit (up to 9
+// digits: nanoseconds); the day's ticks wrap in int64 like every other day-to-tick conversion;
 // month 1..12, day valid for the month (proleptic Gregorian), h < 24, m < 60, s < 60.  castDATE
 // drops the time of day.  Anything else raises an ExecutionError.
 GDV_DEV bool gdv_parse_uint(const gdv_str& s, i32* pos, i32 end, i32 min_digits, i32 max_digits, i64* out) {
@@ -2816,7 +2900,7 @@ GDV_DEV bool gdv_parse_uint(const gdv_str& s, i32* pos, i32 end, i32 min_digits,
   *out = v;
   return n >= min_digits;
 }
-GDV_DEV_BIG i64 gdv_parse_timestamp(gdv_ctx* c, const gdv_str& s, bool date_only) {
+template <i64 TPS> GDV_DEV_BIG i64 gdv_parse_timestamp(gdv_ctx* c, const gdv_str& s, bool date_only) {
   i32 b = 0, e = s.len;
   while (b < e && s.p[b] == (u8)' ') ++b;
   while (e > b && s.p[e - 1] == (u8)' ') --e;
@@ -2825,7 +2909,7 @@ GDV_DEV_BIG i64 gdv_parse_timestamp(gdv_ctx* c, const gdv_str& s, bool date_only
     neg = true;
     ++b;
   }
-  i64 y = 0, mo = 0, d = 0, hh = 0, mi = 0, ss = 0, ms = 0;
+  i64 y = 0, mo = 0, d = 0, hh = 0, mi = 0, ss = 0, ns = 0;
   ok = ok && gdv_parse_uint(s, &b, e, 1, 9, &y);
   ok = ok && b < e && s.p[b] == (u8)'-';
   ++b;
@@ -2849,12 +2933,12 @@ GDV_DEV_BIG i64 gdv_parse_timestamp(gdv_ctx* c, const gdv_str& s, bool date_only
         ++b;
         i32 nd = 0;
         while (b < e && (u32)s.p[b] - (u32)'0' <= 9u) {
-          if (nd < 3) ms = ms * 10 + (i64)((u32)s.p[b] - (u32)'0');
+          if (nd < 9) ns = ns * 10 + (i64)((u32)s.p[b] - (u32)'0');
           ++nd;
           ++b;
         }
         ok = ok && nd >= 1 && b == e;
-        for (; nd < 3; ++nd) ms *= 10;
+        for (; nd < 9; ++nd) ns *= 10;
       }
     }
   }
@@ -2869,12 +2953,16 @@ GDV_DEV_BIG i64 gdv_parse_timestamp(gdv_ctx* c, const gdv_str& s, bool date_only
     gdv_set_error(c, GDV_ERR_CAST_DATE);
     return 0;
   }
-  const i64 day_ms = gdv_days_to_ms(gdv_days_from_civil(y, (i32)mo, (i32)d));
-  if (date_only) return day_ms;
-  return day_ms + ((hh * 60 + mi) * 60 + ss) * 1000 + ms;
+  const i64 day = gdv_days_to_ticks<TPS>(gdv_days_from_civil(y, (i32)mo, (i32)d));
+  if (date_only) return day;
+  const i64 in_day = ((hh * 60 + mi) * 60 + ss) * TPS + ns / (1000000000ll / TPS);
+  return (i64)((u64)day + (u64)in_day);
 }
-GDV_DEV i64 castDATE_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp(c, s, true); }
-GDV_DEV i64 castTIMESTAMP_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp(c, s, false); }
+GDV_DEV i64 castDATE_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp<1000ll>(c, s, true); }
+GDV_DEV i64 castTIMESTAMP_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp<1000ll>(c, s, false); }
+GDV_DEV i64 castTIMESTAMP_s_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp<1ll>(c, s, false); }
+GDV_DEV i64 castTIMESTAMP_us_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp<1000000ll>(c, s, false); }
+GDV_DEV i64 castTIMESTAMP_ns_utf8(gdv_ctx* c, gdv_str s) { return gdv_parse_timestamp<1000000000ll>(c, s, false); }
 
 // ltrim / rtrim / btrim(s, chars): strips glyphs that occur in `chars` (both sides compared as
 // stored bytes: case maps of the operands are ignored for the set test only when they differ per
@@ -2965,10 +3053,6 @@ GDV_DEV i64 crc32_binary(gdv_str s) { return gdv_crc32(s); }
 GDV_DEV f64 degrees_float64(f64 a) { return a * 180.0 / 3.14159265358979323846; }
 GDV_DEV f64 radians_float64(f64 a) { return a * 3.14159265358979323846 / 180.0; }
 // datediff(a, b): whole days between the calendar days of a and b (a - b)
-GDV_DEV i32 datediff_timestamp_timestamp(i64 a, i64 b) {
-  return (i32)(gdv_floordiv(a, 86400000ll) - gdv_floordiv(b, 86400000ll));
-}
-GDV_DEV i32 datediff_date64_date64(i64 a, i64 b) { return datediff_timestamp_timestamp(a, b); }
 
 // ---- virtual pieces: repeat / space / lpad / rpad / reverse ----------------------------------------
 // A periodic view: `total` bytes that repeat the `period` bytes at p (period < 2^20).
@@ -3328,20 +3412,32 @@ GDV_DEV i32 gdv_put_date(u8* scr, i64 days) {
 GDV_DEV gdv_str castVARCHAR_date64_int64(i64 ms, i64 maxlen, u8* scr) {
   return gdv_scratch_str(scr, gdv_put_date(scr, gdv_floordiv(ms, 86400000ll)), maxlen);
 }
-// "YYYY-MM-DD hh:mm:ss.mmm"
-GDV_DEV_BIG gdv_str castVARCHAR_timestamp_int64(i64 ms, i64 maxlen, u8* scr) {
-  const i64 days = gdv_floordiv(ms, 86400000ll);
-  const i64 in_day = (i64)((u64)ms - (u64)gdv_days_to_ms(days));
+// "YYYY-MM-DD hh:mm:ss" plus 0, 3, 6 or 9 fraction digits for s, ms, us, ns (pyarrow's spelling).  The
+// longest spellings, 28 bytes at s ("-292277026596-12-04 15:30:08") and 29 at the other units
+// ("1677-09-21 00:12:43.145224192"), fit GDV_SCRATCH_SLOT (64).
+template <i64 TPS, i32 DIGITS> GDV_DEV_BIG gdv_str gdv_timestamp_text(i64 t, i64 maxlen, u8* scr) {
+  const i64 days = gdv_day_of<TPS>(t);
+  const i64 in_day = gdv_tick_of_day<TPS>(t);
   i32 at = gdv_put_date(scr, days);
   scr[at++] = (u8)' ';
-  at = gdv_put_uint(scr, at, (u64)(in_day / 3600000ll), 2);
+  at = gdv_put_uint(scr, at, (u64)(in_day / (3600ll * TPS)), 2);
   scr[at++] = (u8)':';
-  at = gdv_put_uint(scr, at, (u64)((in_day / 60000ll) % 60), 2);
+  at = gdv_put_uint(scr, at, (u64)((in_day / (60ll * TPS)) % 60), 2);
   scr[at++] = (u8)':';
-  at = gdv_put_uint(scr, at, (u64)((in_day / 1000ll) % 60), 2);
-  scr[at++] = (u8)'.';
-  at = gdv_put_uint(scr, at, (u64)(in_day % 1000ll), 3);
+  at = gdv_put_uint(scr, at, (u64)((in_day / TPS) % 60), 2);
+  if (DIGITS > 0) {
+    scr[at++] = (u8)'.';
+    at = gdv_put_uint(scr, at, (u64)(in_day % TPS), DIGITS);
+  }
   return gdv_scratch_str(scr, at, maxlen);
+}
+GDV_DEV gdv_str castVARCHAR_timestamp_int64(i64 t, i64 maxlen, u8* scr) { return gdv_timestamp_text<1000ll, 3>(t, maxlen, scr); }
+GDV_DEV gdv_str castVARCHAR_timestamp_s_int64(i64 t, i64 maxlen, u8* scr) { return gdv_timestamp_text<1ll, 0>(t, maxlen, scr); }
+GDV_DEV gdv_str castVARCHAR_timestamp_us_int64(i64 t, i64 maxlen, u8* scr) {
+  return gdv_timestamp_text<1000000ll, 6>(t, maxlen, scr);
+}
+GDV_DEV gdv_str castVARCHAR_timestamp_ns_int64(i64 t, i64 maxlen, u8* scr) {
+  return gdv_timestamp_text<1000000000ll, 9>(t, maxlen, scr);
 }
 __device__ const u8 gdv_true_false[9] = {'t', 'r', 'u', 'e', 'f', 'a', 'l', 's', 'e'};
 GDV_DEV gdv_str castVARCHAR_boolean_int64(bool v, i64 maxlen) {

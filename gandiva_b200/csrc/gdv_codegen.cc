@@ -45,8 +45,10 @@ bool IsSupportedType(const DataType& t) {
     case GDV_TYPE_INT64: case GDV_TYPE_FLOAT: case GDV_TYPE_DOUBLE: case GDV_TYPE_STRING:
     case GDV_TYPE_BINARY: case GDV_TYPE_DATE32: case GDV_TYPE_DATE64: case GDV_TYPE_DECIMAL128:
       return true;
-    case GDV_TYPE_TIMESTAMP: case GDV_TYPE_TIME32:
-      return t.precision == 1;  // milliseconds, as in the reference
+    // every Arrow unit: timestamp[s|ms|us|ns], time32[s|ms], time64[us|ns]
+    case GDV_TYPE_TIMESTAMP: return t.precision >= 0 && t.precision <= 3;
+    case GDV_TYPE_TIME32: return t.precision == 0 || t.precision == 1;
+    case GDV_TYPE_TIME64: return t.precision == 2 || t.precision == 3;
     default: return false;
   }
 }
@@ -109,7 +111,7 @@ Status ValidateNode(const Schema& schema, const Node& node) {
         if (!s.ok()) return s;
         params.push_back(c->return_type());
       }
-      const FunctionDef* def = LookupFunction(fn.name(), params);
+      const FunctionDef* def = LookupFunction(fn.name(), params, fn.return_type());
       if (def == nullptr) {
         std::string sig = fn.return_type().ToString() + " " + fn.name() + "(";
         for (size_t i = 0; i < params.size(); ++i)
@@ -547,7 +549,7 @@ class BodyGen {
         const auto& fn = static_cast<const FunctionNode&>(node);
         std::vector<DataType> params;
         for (const auto& c : fn.children()) params.push_back(c->return_type());
-        const FunctionDef* def = LookupFunction(fn.name(), params);
+        const FunctionDef* def = LookupFunction(fn.name(), params, fn.return_type());
         if (def == nullptr || def->nulls != NullMode::kIfNull || (def->flags & (kConcat | kVirtual)) || fn.name() == "nvl")
           return;
         for (const auto& c : fn.children()) ValueStrict(*c, cols);
@@ -586,7 +588,7 @@ class BodyGen {
       const auto& fn = static_cast<const FunctionNode&>(node);
       std::vector<DataType> params;
       for (const auto& c : fn.children()) params.push_back(c->return_type());
-      const FunctionDef* def = LookupFunction(fn.name(), params);
+      const FunctionDef* def = LookupFunction(fn.name(), params, fn.return_type());
       if (def != nullptr && (def->flags & kCanFail)) return true;
       if (ArgGuard(fn) >= 0) return true;
     }
@@ -961,7 +963,7 @@ class BodyGen {
   Val GenFunction(const FunctionNode& fn, std::string* out, int indent) {
     std::vector<DataType> ptypes;
     for (const auto& c : fn.children()) ptypes.push_back(c->return_type());
-    const FunctionDef* def = LookupFunction(fn.name(), ptypes);
+    const FunctionDef* def = LookupFunction(fn.name(), ptypes, fn.return_type());
     const DataType& rt = fn.return_type();
 
     if (def->is_user()) EmitUserFunction(*def);

@@ -99,9 +99,11 @@ const char* DataType::fn_suffix() const {
     case GDV_TYPE_BINARY: return "binary";
     case GDV_TYPE_DATE32: return "date32";
     case GDV_TYPE_DATE64: return "date64";
-    case GDV_TYPE_TIMESTAMP: return "timestamp";
-    case GDV_TYPE_TIME32: return "time32";
-    case GDV_TYPE_TIME64: return "time64";
+    // milliseconds keep the plain names; the other units name theirs (extractYear_timestamp_us, ...)
+    case GDV_TYPE_TIMESTAMP:
+      return precision == 0 ? "timestamp_s" : precision == 2 ? "timestamp_us" : precision == 3 ? "timestamp_ns" : "timestamp";
+    case GDV_TYPE_TIME32: return precision == 0 ? "time32_s" : "time32";
+    case GDV_TYPE_TIME64: return precision == 3 ? "time64_ns" : "time64_us";
     case GDV_TYPE_DECIMAL128: return "decimal128";
     default: return "unknown";
   }

@@ -51,15 +51,18 @@ static bool ParamMatches(const DataType& want, const DataType& got) {
   return true;
 }
 
-const FunctionDef* Registry::Lookup(const std::string& name,
-                                    const std::vector<DataType>& params) const {
+const FunctionDef* Registry::Lookup(const std::string& name, const std::vector<DataType>& params,
+                                    const DataType& ret) const {
+  const FunctionDef* first = nullptr;
   for (const auto& d : defs_) {
     if (d.name != name || d.params.size() != params.size()) continue;
     bool ok = true;
     for (size_t i = 0; i < params.size() && ok; ++i) ok = ParamMatches(d.params[i], params[i]);
-    if (ok) return &d;
+    if (!ok) continue;
+    if (d.ret == ret) return &d;
+    if (first == nullptr) first = &d;
   }
-  return nullptr;
+  return first;
 }
 
 const Registry& Registry::Get() {
@@ -233,8 +236,8 @@ const FunctionDef* FunctionRegistry::Lookup(const std::string& name, const std::
 FunctionRegistry::Scope::Scope(const FunctionRegistry* reg) : prev_(tl_user_functions) { tl_user_functions = reg; }
 FunctionRegistry::Scope::~Scope() { tl_user_functions = prev_; }
 
-const FunctionDef* LookupFunction(const std::string& name, const std::vector<DataType>& params) {
-  if (const FunctionDef* d = Registry::Get().Lookup(name, params)) return d;
+const FunctionDef* LookupFunction(const std::string& name, const std::vector<DataType>& params, const DataType& ret) {
+  if (const FunctionDef* d = Registry::Get().Lookup(name, params, ret)) return d;
   return tl_user_functions != nullptr ? tl_user_functions->Lookup(name, params) : nullptr;
 }
 
@@ -561,6 +564,92 @@ Registry::Registry() {
     Add("concat", std::vector<DataType>(static_cast<size_t>(n), S), S, NullMode::kNever, kConcat);
     Add("concatOperator", std::vector<DataType>(static_cast<size_t>(n), S), S, NullMode::kIfNull, kConcat);
   }
+  AddTimeUnits();
+}
+
+// The twins of every timestamp[ms] / time32[ms] signature at the other units: timestamp[s|us|ns] with the
+// time of day in time32[s], time64[us], time64[ns].  They come after every millisecond signature, so the
+// enumeration keeps its earlier entries and order, and each of them mentions a non-millisecond type.
+// Constructors (castTIMESTAMP, to_timestamp, to_time) take the declared return type's unit: Lookup
+// prefers the def whose return type matches, and their device functions carry the unit in the name
+// (castTIMESTAMP_us_int64, ...).
+void Registry::AddTimeUnits() {
+  const DataType B = boolean(), I32 = int32(), I64 = int64(), F32 = float32(), F64 = float64(), S = utf8();
+  const DataType D64 = date64();
+  static const char* const kUnitName[4] = {"s", "ms", "us", "ns"};
+  auto ts = [](int u) { return DataType(GDV_TYPE_TIMESTAMP, u); };
+  auto tt = [](int u) { return u <= 1 ? DataType(GDV_TYPE_TIME32, u) : DataType(GDV_TYPE_TIME64, u); };
+  auto ctor = [&](const char* name, std::vector<DataType> params, const DataType& ret, int unit, uint32_t flags = 0) {
+    Add(name, std::move(params), ret, NullMode::kIfNull, flags);
+    defs_.back().device_base = std::string(name) + "_" + kUnitName[unit];
+  };
+  static const std::pair<const char*, std::vector<std::string>> kExtract[] = {
+      {"extractYear", {"year"}},       {"extractMonth", {"month"}},     {"extractDay", {"day", "dayofmonth"}},
+      {"extractHour", {"hour"}},       {"extractMinute", {"minute"}},   {"extractSecond", {"second"}},
+      {"extractDoy", {"dayofyear"}},   {"extractDow", {"dayofweek"}},   {"extractQuarter", {"quarter"}},
+      {"extractEpoch", {}}};
+  for (int u : {0, 2, 3}) {
+    const DataType TS = ts(u), TT = tt(u);
+    for (const auto& t : {TS, TT}) {
+      Add("equal", {t, t}, B, NullMode::kIfNull, 0, {"eq", "same"});
+      Add("not_equal", {t, t}, B);
+      Add("less_than", {t, t}, B);
+      Add("less_than_or_equal_to", {t, t}, B);
+      Add("greater_than", {t, t}, B);
+      Add("greater_than_or_equal_to", {t, t}, B);
+      Add("isnull", {t}, B, NullMode::kNever);
+      Add("isnotnull", {t}, B, NullMode::kNever);
+      Add("is_distinct_from", {t, t}, B, NullMode::kNever);
+      Add("is_not_distinct_from", {t, t}, B, NullMode::kNever);
+      Add("hash32", {t}, I32, NullMode::kNever, 0, {"hash", "hash32AsDouble"});
+      Add("hash32", {t, I32}, I32, NullMode::kNever, 0, {"hash32AsDouble"});
+      Add("hash64", {t}, I64, NullMode::kNever, 0, {"hash64AsDouble"});
+      Add("hash64", {t, I64}, I64, NullMode::kNever, 0, {"hash64AsDouble"});
+      Add("nvl", {t, t}, t, NullMode::kInternal);
+    }
+    Add("castBIGINT", {TS}, I64);
+    Add("castDATE", {TS}, D64);
+    for (const auto& e : kExtract) Add(e.first, {TS}, I64, NullMode::kIfNull, 0, e.second);
+    Add("extractWeek", {TS}, I64, NullMode::kIfNull, 0, {"weekofyear", "yearweek"});
+    for (const char* f : {"extractDecade", "extractCentury", "extractMillennium"}) Add(f, {TS}, I64);
+    for (const char* un : {"Second", "Minute", "Hour", "Day", "Week", "Month", "Quarter", "Year", "Decade",
+                           "Century", "Millennium"})
+      Add(std::string("date_trunc_") + un, {TS}, TS);
+    Add("last_day", {TS}, D64);
+    for (const char* f : {"timestampaddSecond", "timestampaddMinute", "timestampaddHour", "timestampaddDay",
+                          "timestampaddWeek", "timestampaddMonth", "timestampaddQuarter", "timestampaddYear"}) {
+      Add(f, {I32, TS}, TS);
+      Add(f, {I64, TS}, TS);
+      Add(f, {TS, I32}, TS);
+      Add(f, {TS, I64}, TS);
+    }
+    Add("add_months", {TS, I32}, TS);
+    Add("add_months", {TS, I64}, TS);
+    Add("date_add", {TS, I32}, TS);
+    Add("date_sub", {TS, I32}, TS);
+    for (const char* f : {"timestampdiffSecond", "timestampdiffMinute", "timestampdiffHour", "timestampdiffDay",
+                          "timestampdiffWeek", "timestampdiffMonth", "timestampdiffQuarter", "timestampdiffYear"})
+      Add(f, {TS, TS}, I32);
+    Add("months_between", {TS, TS}, F64);
+    Add("datediff", {TS, TS}, I32);
+    Add("castTIME", {TS}, TT);
+    Add("extractHour", {TT}, I64, NullMode::kIfNull, 0, {"hour"});
+    Add("extractMinute", {TT}, I64, NullMode::kIfNull, 0, {"minute"});
+    Add("extractSecond", {TT}, I64, NullMode::kIfNull, 0, {"second"});
+    Add("castVARCHAR", {TS, I64}, S, NullMode::kIfNull, kScratch);
+    // constructors in this unit
+    ctor("castTIMESTAMP", {I64}, TS, u);
+    ctor("castTIMESTAMP", {D64}, TS, u);
+    ctor("castTIMESTAMP", {S}, TS, u, kCanFail);
+    for (const auto& t : {I32, I64, F32, F64}) {
+      ctor("to_timestamp", {t}, TS, u);
+      ctor("to_time", {t}, TT, u);
+    }
+  }
+  // unit conversions between any two different units
+  for (int to = 0; to < 4; ++to)
+    for (int from = 0; from < 4; ++from)
+      if (from != to) ctor("castTIMESTAMP", {ts(from)}, ts(to), to);
 }
 
 }  // namespace gdv

@@ -53,8 +53,10 @@ struct FunctionDef {
 class Registry {
  public:
   static const Registry& Get();
-  // Exact match on name and parameter types (decimal: id only; timestamp/time: unit too).
-  const FunctionDef* Lookup(const std::string& name, const std::vector<DataType>& params) const;
+  // Exact match on name and parameter types (decimal: id only; timestamp/time: unit too).  Among the
+  // defs that match, the one whose return type equals `ret` (the type the call site declares) wins,
+  // else the first: constructors such as castTIMESTAMP(int64) exist once per result unit.
+  const FunctionDef* Lookup(const std::string& name, const std::vector<DataType>& params, const DataType& ret) const;
   const std::vector<FunctionDef>& all() const { return defs_; }
 
  private:
@@ -62,6 +64,7 @@ class Registry {
   void Add(const std::string& name, std::vector<DataType> params, DataType ret,
            NullMode nulls = NullMode::kIfNull, uint32_t flags = 0,
            const std::vector<std::string>& aliases = {});
+  void AddTimeUnits();
   std::vector<FunctionDef> defs_;
 };
 
@@ -117,7 +120,8 @@ class FunctionRegistry {
 // Text of gdv_raise(ctx, "message"), written into a kernel before its first user function that can raise.
 extern const char kUserRaiseHelper[];
 
-// Built-ins first, then the registry of the enclosing FunctionRegistry::Scope.
-const FunctionDef* LookupFunction(const std::string& name, const std::vector<DataType>& params);
+// Built-ins first, then the registry of the enclosing FunctionRegistry::Scope.  `ret` is the return type
+// the call site declares (see Registry::Lookup).
+const FunctionDef* LookupFunction(const std::string& name, const std::vector<DataType>& params, const DataType& ret);
 
 }  // namespace gdv
